@@ -39,8 +39,7 @@ def parse():
     ap.add_argument("--steps", type=int, default=100)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--batch", type=int, default=32,
-                    help="frames per step.  profiles/r02_t7_frames_per_step_sweep.txt: 64 is +2 %% over 32 on one box, but the worst parity "
-                         "case measured at 64 (recipe B, frames 0/32/63) is 5.3e-4 where 32 gives 3.6e-4 - the default keeps the wider margin")
+                    help="frames per step (the parity tests gate 16, 32 and 64)")
     ap.add_argument("--mode", default="parity", choices=["parity", "fast"])
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--variant", default="large", choices=["large", "normal"],
@@ -49,6 +48,11 @@ def parse():
     ap.add_argument("--width", type=int, default=512)
     ap.add_argument("--gather", default="auto", choices=["auto", "ce", "nccl"],
                     help="N > 1: how rendered frames reach every rank (parallel.ShardedRenderer)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the timed path returned in its last step to DIR/<name>.npy, 64 MB "
+                         "in all: frames.npy (float32) = a fixed, seeded sample of up to 16 of its [B,3,H,W] frames, as many as fit "
+                         "(frame_indices.npy says which); if one frame alone exceeds 64 MB, frame0_pixels.npy = a fixed, seeded "
+                         "sample of the first frame's values (frame0_pixel_indices.npy: flat indices into [3,H,W])")
     ap.add_argument("--clip-frames", type=int, default=10000,
                     help="N > 1: also render one clip of exactly this many frames and report it as clip_run (BASELINE.json "
                          "configs[3]: 10000 synthetic frames, frame-sharded; 0 = skip)")
@@ -69,7 +73,7 @@ def config_dict(args, world: int) -> dict:
                     "per step (BASELINE.json configs[1]/[3]; the one-frame-per-call rate of demo.py is reported as single_frame), "
                     + ("single GPU" if world == 1 else f"frame-sharded over {world} GPUs, every rank receives every frame"),
         "variant": v, "batch": B, "height": H, "width": W, "precision_mode": args.mode, "parallelism": f"dp{world}",
-        "l2": "per-step working set (weights 0.24-0.49 GB + activations > 1 GB) exceeds the 126 MB L2; input batches rotate "
+        "l2": "per-step working set (weights 0.24-0.49 GB + activations > 1 GB) exceeds the 50 MB L2; input batches rotate "
               "over a pool",
     }
 
@@ -78,8 +82,8 @@ def measured_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1451.7), d.get("hbm_gbs", 6572.9), "MEASURED_PEAKS.json (sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("bf16_tflops_sustained", 989.0), d.get("hbm_gbs", 3350.0), "MEASURED_PEAKS.json (sustained bf16)"
+    return 989.0, 3350.0, "H100 SXM data sheet (dense bf16, HBM3; not measured)"
 
 
 def host_cpu_info() -> dict:
@@ -232,7 +236,7 @@ def timed_ms(fn, n: int, warm: int = 3) -> float:
 
 
 def library_baseline(variant: str, batch: int, h: int, w: int) -> dict:
-    """PyTorch eager + cuDNN on the same GPU, same batch: what the unmodified reference module would execute on this B200
+    """PyTorch eager + cuDNN on the same GPU, same batch: what the unmodified reference module would execute on this H100
     (base_model.py:46-47 sets cudnn.benchmark).  A library baseline beside the hand-written kernels, never the product path."""
     from oracle import f2f_oracle as O
     torch.backends.cudnn.benchmark = True
@@ -292,6 +296,34 @@ def side_config(variant: str, mode: str, batch: int, h: int, w: int, tflops_peak
     return res
 
 
+DUMP_BYTES = 64 << 20        # cap of everything --dump-outputs writes
+
+
+def dump_outputs(out_dir: str, frames: torch.Tensor) -> None:
+    """The frames the timed path returned in its last step (N > 1: the gathered clip), as float32 .npy files within
+    DUMP_BYTES: a fixed, seeded sample of whole frames (up to 16; 48 MB at 512x512), or, where a single frame exceeds the cap,
+    a fixed, seeded sample of pixels of the first frame.  The same arguments give the same sample, so two builds compare
+    output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    n = frames.shape[0]
+    per_frame = frames[0].numel() * 4
+    rng = np.random.default_rng(0)
+    budget = DUMP_BYTES - 4096                                  # room for the .npy headers
+    if per_frame + 8 <= budget:
+        k = min(n, 16, budget // (per_frame + 8))
+        idx = np.sort(rng.choice(n, size=k, replace=False))
+        np.save(os.path.join(out_dir, "frames.npy"), frames[torch.from_numpy(idx).to(frames.device)].float().cpu().numpy())
+        np.save(os.path.join(out_dir, "frame_indices.npy"), idx.astype(np.float64))
+    else:
+        flat = frames[0].reshape(-1)
+        # values plus their float64 flat indices: 12 bytes per sampled pixel value
+        k = min(flat.numel(), budget // 12)
+        idx = np.sort(rng.choice(flat.numel(), size=k, replace=False))
+        np.save(os.path.join(out_dir, "frame0_pixels.npy"), flat[torch.from_numpy(idx).to(frames.device)].float().cpu().numpy())
+        np.save(os.path.join(out_dir, "frame0_pixel_indices.npy"), idx.astype(np.float64))
+
+
 def main():
     global _REAL_STDOUT
     args = parse()
@@ -309,7 +341,7 @@ def main():
         run_reference(args, rank)
         return
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py needs a B200: there is no CPU path for the product arm (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py needs an H100: there is no CPU path for the product arm (use --impl reference for the CPU arm)")
     import torch.distributed as dist
     from oracle import f2f_oracle as O
     from livespeechportraits_b200.parallel import ShardedRenderer, partition
@@ -407,6 +439,8 @@ def main():
                 errs.append(oracle_err(clip_all[g:g + 1], r, st_, j))
             parity_err = max(errs)
             parity_note = f"frames (rank, step, index) {picks} of the gathered clip on rank 0 vs the oracle"
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last if world == 1 else clip_all)
     ms_total = e0.elapsed_time(e1)
     ms_step_local = ms_total / K
     clocks = sampler.stop(t_wall0, t_wall1) if rank == 0 else None
@@ -429,7 +463,7 @@ def main():
     frames = B * K * world
     value = frames / (ms_total / 1e3)
 
-    # ---- roofline of the dominant kernel family (the tcgen05 convs), from the per-launch events of the timed workload
+    # ---- roofline of the dominant kernel family (the wgmma convs), from the per-launch events of the timed workload
     rows = net.layer_table(H, W)
     conv_ms = prof_ms[1:]
     groups = {}
@@ -451,25 +485,15 @@ def main():
             f *= 4.0 / 9.0
         exec_flops += f * (3.0 if args.mode == "parity" else 1.0)
     top = sorted(groups.items(), key=lambda kv: -kv[1]["ms"])[:6]
-    traffic = None
-    tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(tpath):
-        try:
-            cand_t = [t for t in json.load(open(tpath)) if t.get("batch") == B and t.get("mode") == args.mode and t.get("variant") == VARIANT]
-            traffic = cand_t[0] if cand_t else None
-        except Exception:
-            traffic = None
     roofline = {
-        "bound": "tensor", "kernel": "lspg::conv_pair_kernel / conv_umma_kernel / conv_patch_kernel (all conv launches of one step)",
+        "bound": "tensor", "kernel": "lspg::conv_umma_kernel / conv_patch_kernel (all conv launches of one step)",
         "achieved": achieved, "peak": tflops_peak, "unit": "TFLOP/s", "frac": achieved / tflops_peak, "peak_source": peak_src,
-        "traffic": traffic.get("dram_bytes_per_launch") if traffic else None,
-        "traffic_detail": traffic,
         "algorithmic_flops_per_step": flops_step, "kernel_ms_per_step": conv_ms_timed,
         "kernel_ms_per_step_event_pass": tot_ms, "pack_input_ms": prof_ms[0], "forwards_profiled": prof_n,
         "executed_tflops": exec_flops / (conv_ms_timed / 1e3) / 1e12 if conv_ms_timed > 0 else None,
         "executed_frac": (exec_flops / (conv_ms_timed / 1e3) / 1e12) / tflops_peak if conv_ms_timed > 0 else None,
         "note": "achieved = reference-conv FLOPs / time of the conv launches in the timed region; parity mode issues "
-                "3 tcgen05 MMAs per K step (hi*hi, hi*lo, lo*hi), so executed_* is the tensor-pipe view",
+                "3 wgmma MMAs per K step (hi*hi, hi*lo, lo*hi), so executed_* is the tensor-pipe view",
         "top_groups": [{"group": k, "ms": round(v["ms"], 4), "launches": v["launches"],
                         "tflops": round(v["flops"] / (v["ms"] / 1e3) / 1e12, 1) if v["ms"] > 0 else None} for k, v in top],
     }
@@ -717,7 +741,7 @@ def main():
         line = {
             "metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": K, "warmup": Wm,
             "ms_per_step": ms_total / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "bf16" if args.mode == "fast" else "fp16 hi+lo split operands (3 tcgen05 MMAs per K step), fp32 accumulate",
+            "dtype": "bf16" if args.mode == "fast" else "fp16 hi+lo split operands (3 wgmma MMAs per K step), fp32 accumulate",
             "data": "synthetic (seeded weights with the reference's init distribution - no checkpoint ships; seeded inputs)",
             "config": config_dict(args, world),
             "max_abs_err_vs_oracle": parity_err, "max_abs_err_note": parity_note,

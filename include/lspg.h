@@ -1,5 +1,5 @@
 /*
- * lspg.h - C ABI of the B200-native Feature2Face generator (LiveSpeechPortraits render hot path).
+ * lspg.h - C ABI of the H100-native Feature2Face generator (LiveSpeechPortraits render hot path).
  *
  * The reference has no native code and no FFI: its "plugin boundary" for this path is the Python class
  * models/feature2face_G.py:Feature2Face_G (ctor(opt) :8-21, forward(input) :27-34) held by
@@ -10,7 +10,7 @@
  *
  * Conventions: plain C types only; every function returns 0 on success or a negative LSPG_E* code and
  * records a message retrievable with lspg_last_error() (thread-local).  No CPU compute path exists:
- * forward needs an sm_100 device and fails loudly otherwise.  One handle per device; calls on one handle
+ * forward needs an sm_90 device and fails loudly otherwise.  One handle per device; calls on one handle
  * must be serialised by the caller.  All device work is enqueued on the caller's stream; nothing
  * synchronises or allocates inside lspg_forward once the (B,H,W,mode,workspace) plan is cached.
  */
@@ -26,7 +26,7 @@ extern "C" {
 
 #define LSPG_OK 0
 #define LSPG_EINVAL (-1)     /* bad argument / unsupported shape */
-#define LSPG_ENODEV (-2)     /* no sm_100 device / host-only handle */
+#define LSPG_ENODEV (-2)     /* no sm_90 device / host-only handle */
 #define LSPG_ECUDA (-3)      /* CUDA runtime or driver error */
 #define LSPG_ESTATE (-4)     /* weights not loaded, workspace too small, ... */
 #define LSPG_ENOMEM (-5)
@@ -127,22 +127,20 @@ typedef struct lspg_layer_info {
 } lspg_layer_info;
 
 /* Tiling / kernel choice of one layer for a problem size, as the launch plan will make it (host logic only; works on a
- * host-only handle, where the SM count defaults to 148).  Lets the CPU tests pin the planner. */
+ * host-only handle, where the SM count defaults to 132, H100 SXM).  Lets the CPU tests pin the planner. */
 typedef struct lspg_layer_geo {
-  int kernel;            /* 0 conv_umma_kernel (one box per tap), 1 conv_patch_kernel, 2 conv_pair_kernel (cta_group::2) */
+  int kernel;            /* 0 conv_umma_kernel (one box per tap), 1 conv_patch_kernel (halo patch) */
   int bn;                /* N tile */
   int tile_w, tile_h, tile_n;   /* output tile = tile_w x tile_h pixels x tile_n images = 128 rows */
   int m_tiles, n_tiles, n_phases;
   int n_split, split_len, k_items;   /* split-K: K loop of k_items cut into n_split ranges of split_len */
-  int ctas;              /* CTAs launched = min(tiles * n_split, SMs), even for the pair kernel */
-  int64_t partial_bytes; /* fp32 split-K partials this layer needs in the scratch region (0 for a cluster split) */
-  int cluster_split;     /* > 0: the n_split CTAs of a tile are one thread-block cluster and reduce through distributed shared
-                            memory (no finisher launch); then n_split == cluster_split in {2, 4, 8} */
+  int ctas;              /* CTAs launched = min(tiles * n_split, SMs) */
+  int64_t partial_bytes; /* fp32 split-K partials this layer needs in the scratch region (summed by the finisher kernel) */
 } lspg_layer_geo;
 int lspg_debug_layer_geo(lspg_handle h, int layer, int batch, int height, int width, lspg_layer_geo* out);
 
 /* Test hook (host only, no device): q = n / d computed exactly as the kernels' tile decode does it (multiply-high by a
- * launch-time constant, csrc/conv_umma.cuh make_fast_div / fast_div); valid for n < 2^31, d >= 1. */
+ * launch-time constant, csrc/conv_wgmma.cuh make_fast_div / fast_div); valid for n < 2^31, d >= 1. */
 int lspg_debug_fast_div(uint32_t n, uint32_t d, uint32_t* q);
 
 int lspg_num_layers(lspg_handle h, int* out);
@@ -160,7 +158,7 @@ int lspg_tensor_shape(lspg_handle h, int id, int height, int width, int* c, int*
  * recent forward to host memory. */
 int lspg_debug_read_tensor(lspg_handle h, int id, int limb, uint16_t* dst, int64_t count);
 /* Debug: with LSPG_TRACE_LAYER=<i> in the environment the conv kernel of layer i stamps clock64() at its pipeline
- * milestones (conv_umma.cuh: kTraceSlots values per CTA, 256 CTAs); this copies them out. */
+ * milestones (conv_wgmma.cuh: kTraceSlots values per CTA, 256 CTAs); this copies them out. */
 int lspg_debug_read_trace(lspg_handle h, uint64_t* dst, int64_t count);
 /* CUDA-graph bookkeeping since lspg_create: graphs captured + instantiated, in-place I/O pointer updates, and re-captures
  * forced by a failed update (expected 0). */

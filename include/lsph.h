@@ -1,5 +1,5 @@
 /*
- * lsph.h - C ABI of the B200-native Audio2Headpose generation loop (LiveSpeechPortraits, SURVEY.md 8f row N4).
+ * lsph.h - C ABI of the H100-native Audio2Headpose generation loop (LiveSpeechPortraits, SURVEY.md 8f row N4).
  *
  * What it replaces: the autoregressive loop of models/audio2headpose_model.py:169-187 - per generated frame one
  * Audio2Headpose.forward (models/audio2headpose.py:41-53: audio_downsample of a 255-row window + a 255-step WaveNet,
@@ -10,7 +10,7 @@
  * conditioning convolutions, which do not depend on the generated history, are hoisted out of the loop as three GEMMs, and
  * Sample_GMM runs on the device with the random draws passed in.
  *
- * Conventions as in lspg.h: plain C types, 0 or a negative LSPG_E* code, message in lsph_last_error(); sm_100 only,
+ * Conventions as in lspg.h: plain C types, 0 or a negative LSPG_E* code, message in lsph_last_error(); sm_90 only,
  * no CPU path.  The Python binding (livespeechportraits_b200/headpose.py) keeps the reference's
  * generate_sequences(audio_feats, pre_headpose, fill_zero, sigma_scale, opt) signature.
  */

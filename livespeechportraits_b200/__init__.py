@@ -1,4 +1,4 @@
-"""B200-native implementation of LiveSpeechPortraits' per-frame renderer (``Feature2Face_G``) and the steps either
+"""H100-native implementation of LiveSpeechPortraits' per-frame renderer (``Feature2Face_G``) and the steps either
 side of it.  Public names:
 
 * ``Feature2Face_G`` / ``install`` - drop-in for ``models/feature2face_G.py`` (generator.py)

@@ -1,4 +1,4 @@
-"""Compile the CUDA extension in-tree for sm_100a (nvcc cross-compiles without a GPU).
+"""Compile the CUDA extension in-tree for sm_90a (nvcc cross-compiles without a GPU).
 
 ``python -m livespeechportraits_b200.build`` or ``build_library()`` produces
 ``livespeechportraits_b200/liblspg.so`` - a plain C-ABI shared library (include/lspg.h, include/lsph.h), statically linked
@@ -16,11 +16,11 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "liblspg.so")
 SOURCES = ["lspg.cu", "lsph.cu"]
-HEADERS = ["conv_umma.cuh", "ptx.cuh", "aux_kernels.cuh", "raster.cuh", os.path.join("..", "..", "include", "lspg.h"),
+HEADERS = ["conv_wgmma.cuh", "ptx.cuh", "aux_kernels.cuh", "raster.cuh", os.path.join("..", "..", "include", "lspg.h"),
            os.path.join("..", "..", "include", "lsph.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-shared", "-Xcompiler", "-fPIC",
     "-cudart", "static",

@@ -1,8 +1,8 @@
-// C-ABI implementation of the B200-native Feature2Face generator (see include/lspg.h).
+// C-ABI implementation of the H100-native Feature2Face generator (see include/lspg.h).
 //
 // Host side: network structure (mirrors models/networks.py:554-675 of the reference), weight packing with
 // eval-BatchNorm folding, activation-tensor planning, TMA descriptor construction, launch sequencing.
-// Device side: conv_umma.cuh (tcgen05/TMA implicit-GEMM conv) and aux_kernels.cuh (input packer).
+// Device side: conv_wgmma.cuh (wgmma/TMA implicit-GEMM conv) and aux_kernels.cuh (input packer).
 #include <cuda.h>
 #include <cuda_runtime.h>
 
@@ -23,7 +23,7 @@
 #include "../../include/lspg.h"
 #include "aux_kernels.cuh"
 #include "raster.cuh"
-#include "conv_umma.cuh"
+#include "conv_wgmma.cuh"
 
 namespace {
 
@@ -108,10 +108,8 @@ struct PlanLayer {
   int bn = 64;
   int grid = 1;
   bool patch = false;     // conv_patch_kernel (halo patch per chunk) instead of conv_umma_kernel (one box per tap)
-  bool pair = false;      // conv_pair_kernel (cta_group::2)
   int cluster = 1;        // CTAs per cluster sharing B stages by TMA multicast (patch mode only)
   bool split = false;     // split-K: conv kernel writes fp32 partials, splitk_reduce_kernel finishes
-  int csplit = 0;         // split-K inside a cluster of this many CTAs (no finisher)
   ReduceParams red;
   int red_blocks = 0;
 };
@@ -155,7 +153,7 @@ struct lspg_ctx {
   EncodeTiledFn encode = nullptr;
   std::map<std::tuple<int, int, int, int, void*>, std::unique_ptr<Plan>> plans;
   Plan* last_plan = nullptr;
-  int num_sms_or_default() const { return num_sms > 0 ? num_sms : 148; }
+  int num_sms_or_default() const { return num_sms > 0 ? num_sms : 132; }   // H100 SXM
   cudaStream_t capture_stream = nullptr;
   long long n_captures = 0, n_io_updates = 0, n_recaptures = 0;   // graph bookkeeping (lspg_graph_stats)
   const void* tail_func = nullptr;           // host stub of the tail kernel the last enqueue launched
@@ -451,8 +449,6 @@ size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 int nl_of(int mode) { return mode == LSPG_MODE_PARITY ? 2 : 1; }
 
-// conv_pair_kernel variant with stacked [B_hi; B_lo] operands (parity mode, N tile 64); see PairCfg
-bool pair_stacked(int bn, int NL) { return bn == 64 && NL == 2; }
 
 size_t tensor_bytes_one_limb(const TensorInfo& t, int B, int H, int W) {
   return static_cast<size_t>(B) * (H >> t.shift) * (W >> t.shift) * t.channels * 2;
@@ -473,8 +469,6 @@ struct Geo {
   int k_items;                 // K-loop length: K blocks (v1) or (source, chunk) items (patch)
   int n_split, split_len;
   size_t partial_bytes;
-  bool pair;                   // conv_pair_kernel: cta_group::2 UMMA over a 2-CTA cluster (wide layers)
-  int csplit;                  // > 0: split-K inside a thread-block cluster of this many CTAs (DSMEM reduction, no finisher)
 };
 
 Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
@@ -486,7 +480,7 @@ Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
   g.th = 128 / g.tw;
   if (g.th > g.hs) g.th = g.hs;
   g.nb = 128 / (g.tw * g.th);
-  // patch mode needs 8-pixel-wide tiles (one UMMA 8-row group = one image row of the halo patch)
+  // patch mode needs 8-pixel-wide tiles (one 8-row core-matrix group of the wgmma A operand = one image row of the halo patch)
   g.patch = !no_patch && L.kind != K_S2 && g.ws >= 8 && g.hs >= 16;
   if (g.patch) { g.tw = 8; g.th = 16; g.nb = 1; }
   g.m_tiles = (g.ws / g.tw) * (g.hs / g.th) * ((B + g.nb - 1) / g.nb);
@@ -497,60 +491,17 @@ Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
   // per-tap kernel below 16^2: the N=128 tile halves the A traffic per MAC (the kernel is shared-memory bound) and split-K
   // restores the CTA count
   if (!g.patch && L.kind != K_TAIL && L.cout_pad % 128 == 0 && g.m_tiles >= 8) g.bn = 128;
-  // CTA-pair kernel for the wide layers: N tile 256 (or 128), two neighbouring M tiles per cluster
-  static const bool no_pair = getenv("LSPG_NO_PAIR") != nullptr;
-  g.pair = false;
-  if (!no_pair && g.patch && (L.kind == K_S1 || L.kind == K_UP) && L.cout_pad % 64 == 0 && g.m_tiles % 2 == 0) {
-    const int sms = h->num_sms_or_default();
-    int bnp = 0;
-    // a pair tile runs the tensor pipe at full rate while the N=64 single-CTA tile is shared-memory bound at ~60 %,
-    // so the pair kernel already wins when its tiles fill about two thirds of the SMs
-    const int enough = sms * 2 / 3;
-    // Tiles are equal-sized and statically strided over sms/2 clusters, so a launch costs ceil(pairs / clusters) waves of
-    // one tile each: 256 pairs of N=256 tiles on 74 clusters are 4 waves (3.46 needed), the same work as 512 pairs of N=128
-    // tiles is 7 half-sized waves (-12.5 %).  Take the N tile with the lower wave cost; ties go to the wider tile (fewer
-    // A operand reads).
-    auto wave_cost = [&](int bn) {
-      const long long pairs = static_cast<long long>(g.m_tiles) * (L.cout_pad / bn) * L.n_phases / 2;
-      const long long clusters = sms / 2;
-      return (pairs + clusters - 1) / clusters * bn;
-    };
-    if (L.cout_pad % 256 == 0 && g.m_tiles * (L.cout_pad / 256) * L.n_phases >= sms)
-      bnp = wave_cost(128) < wave_cost(256) ? 128 : 256;
-    else if (L.cout_pad % 128 == 0 && g.m_tiles * (L.cout_pad / 128) * L.n_phases >= enough) bnp = 128;
-    else if (L.cout_pad == 64 && g.m_tiles * L.n_phases >= enough) bnp = 64;
-    if (bnp) { g.pair = true; g.bn = bnp; }
-  }
   g.n_tiles = L.cout_pad / g.bn;
   g.tiles_per_split = g.m_tiles * g.n_tiles * L.n_phases;
-  g.n_split = 1; g.split_len = g.k_items; g.partial_bytes = 0; g.csplit = 0;
+  g.n_split = 1; g.split_len = g.k_items; g.partial_bytes = 0;
   const int sms = h->num_sms_or_default();
-  if (!no_split && !g.pair && L.kind != K_TAIL && g.tiles_per_split * 2 <= sms) {
+  if (!no_split && L.kind != K_TAIL && g.tiles_per_split * 2 <= sms) {
     const int min_len = g.patch ? 1 : 4;                       // at least 4 K blocks (v1) / 1 chunk of all taps per split
     int want = sms / g.tiles_per_split;                        // floor: tiles x splits stay within one wave
     int max_split = g.k_items / min_len;
     if (max_split < 1) max_split = 1;
     if (want > max_split) want = max_split;
-    // Cluster split-K: the 2 / 4 / 8 CTAs of a tile form a cluster, exchange their partial rows through distributed shared
-    // memory and finish the tile themselves - no partials in global memory, no finisher launch.  Needs exactly `cs`
-    // non-empty K ranges and tiles x cs CTAs in one wave.
-    // Measured on one B200 (profiles/r02_t3_ab_cluster_split.txt, alternating runs): 32 frames per step 15.57-15.67 ms with
-    // the cluster reduction vs 15.77-15.82 ms with finisher kernels (-1 %); one frame per call 1.283 vs 1.262 ms (+1.7 %: at
-    // batch 1 a cluster of 8 leaves 64 CTAs streaming the layer's weights where 18 finisher-splits keep 144 busy, and under
-    // PDL the finisher launches were almost free).  So clusters from 8 frames up, finishers below; LSPG_CLUSTER_SPLIT=0/1
-    // forces either for A/B runs.
-    static const int csplit_env = [] { const char* e = getenv("LSPG_CLUSTER_SPLIT"); return e ? atoi(e) : -1; }();
-    const bool use_csplit = csplit_env >= 0 ? csplit_env != 0 : B >= 8;
-    if (use_csplit && want > 1) {
-      for (int cs : {8, 4, 2}) {
-        if (cs > want) continue;
-        const int len = (g.k_items + cs - 1) / cs;
-        if ((g.k_items + len - 1) / len != cs) continue;
-        g.csplit = cs; g.n_split = cs; g.split_len = len;
-        break;
-      }
-    }
-    if (!g.csplit && want > 1) {
+    if (want > 1) {
       g.split_len = (g.k_items + want - 1) / want;
       g.n_split = (g.k_items + g.split_len - 1) / g.split_len;
       if (g.n_split > 1) g.partial_bytes = static_cast<size_t>(g.n_split) * g.tiles_per_split * kTileM * g.bn * sizeof(float);
@@ -660,20 +611,6 @@ int patch_tps(int bn, int NL, bool tail) {   // must mirror PatchCfg::kTPS
   return NL == 1 ? 3 : 2;
 }
 
-uint32_t make_idesc(int bn, int m, bool f16) {
-  // cute::UMMA::InstrDescriptor bit layout: c_format[4,6)=1 (F32), a_format[7,10) and b_format[10,13): 0 = F16, 1 = BF16,
-  // a/b major [15],[16] = 0 (K-major), n_dim[17,23) = N>>3, m_dim[24,29) = M>>4
-  uint32_t d = 0;
-  d |= 1u << 4;
-  if (!f16) {
-    d |= 1u << 7;
-    d |= 1u << 10;
-  }
-  d |= static_cast<uint32_t>(bn >> 3) << 17;
-  d |= static_cast<uint32_t>(m >> 4) << 24;
-  return d;
-}
-
 int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* workspace) {
   const int NL = nl_of(mode);
   P->batch = B; P->height = H; P->width = W; P->mode = mode; P->workspace = workspace;
@@ -695,8 +632,8 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     const Geo g = layer_geo(h, L, B, H, W);
     const int Hs = g.hs, Ws = g.ws;
     const int tw = g.tw, th = g.th, nb = g.nb;
-    // Measured on B200 (gpurun bringup2): the UMMA swizzle phase follows the absolute smem address, so a 128-byte-shifted
-    // start needs NO descriptor base offset (setting it corrupts the result).
+    // The tensor core's swizzle phase follows the absolute smem address (as TMA's does), so a 128-byte-shifted start
+    // needs no descriptor base offset.
     pl.patch = g.patch;
     int abox_w = tw, abox_h = th, abox_n = nb;
     if (pl.patch) {
@@ -731,26 +668,15 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     p.fd_tiles_y = make_fast_div(p.tiles_y);
     p.n_split = g.n_split; p.split_len = g.split_len;
     p.total_tiles = g.tiles_per_split * g.n_split;
-    if (g.pair) {
-      const int n_items = g.k_items * L.n_taps;                           // weight tiles per output tile
-      const int stage = (pair_stacked(g.bn, NL) ? 3 : NL) * (g.bn / 2) * 128;
-      const int cap = std::min(16, (kSmemBudget - 1024 - 5120 - 2 * NL * kPatchStride) / stage);
-      p.b_resident = (L.n_phases == 1 && g.n_tiles == 1 && n_items <= cap) ? 1 : 0;
-    }
     p.partial = reinterpret_cast<float*>(ws_scratch);
-    // Split-K is two-pass: raw fp32 partials, then splitk_reduce_kernel.  (Measured on B200 in round 1: letting the
-    // last-arriving CTA sum the partials in-kernel was slower - one CTA's epilogue threads reduce a tile far more slowly
-    // than a grid of them - so that variant was removed.)
-    pl.split = g.n_split > 1 && g.csplit == 0;
-    pl.csplit = g.csplit;
-    p.cluster_split = g.csplit ? 1 : 0;
+    // Split-K without a cluster is two-pass: raw fp32 partials, then splitk_reduce_kernel (a grid of threads sums a tile
+    // far faster than the epilogue threads of the last-arriving CTA could).
+    pl.split = g.n_split > 1;
     p.n_taps = L.n_taps; p.n_src = L.n_src;
     p.chunks[0] = L.cin[0] / 64; p.chunks[1] = L.n_src == 2 ? L.cin[1] / 64 : 0;
     p.relu = L.relu; p.has_res = L.res >= 0 ? 1 : 0;
     p.batch = B; p.hs = Hs; p.ws = Ws;
     const bool f16 = NL > 1;                  // PARITY operands are fp16 limbs, FAST operands bf16
-    p.idesc = make_idesc(pl.bn, g.pair ? 256 : kTileM, f16);
-    p.idesc2 = make_idesc(2 * pl.bn > 256 ? 256 : 2 * pl.bn, g.pair ? 256 : kTileM, f16);
     p.scale = f16 ? L.d_scale_par : L.d_scale; p.shift = L.d_shift; p.out_f32 = nullptr;
     memcpy(p.tap_map, L.tap_map, sizeof(p.tap_map));
     memcpy(p.tap_dx, L.tap_dx, sizeof(p.tap_dx));
@@ -774,27 +700,18 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     for (int q = used; q < 4; ++q) p.a[q] = p.a[0];
     if (pl.patch) {
       static const bool no_cluster = getenv("LSPG_NO_CLUSTER") != nullptr;
-      pl.pair = g.pair;
-      pl.cluster = (g.pair || (!no_cluster && g.n_split == 1 && g.m_tiles % 2 == 0 && g.tiles_per_split >= h->num_sms)) ? 2 : 1;
-      if (pl.cluster == 1 && NL == 1 && !pl.pair) rc = make_weight_map_taps(h, &p.w, L, pl.bn, patch_tps(pl.bn, NL, L.kind == K_TAIL), NL);
+      pl.cluster = ((!no_cluster && g.n_split == 1 && g.m_tiles % 2 == 0 && g.tiles_per_split >= h->num_sms)) ? 2 : 1;
+      if (pl.cluster == 1 && NL == 1) rc = make_weight_map_taps(h, &p.w, L, pl.bn, patch_tps(pl.bn, NL, L.kind == K_TAIL), NL);
       else rc = make_weight_map_taps(h, &p.w, L, pl.bn / pl.cluster, 1, NL);      // per-tap boxes (row slice per CTA when multicasting)
       if (rc) return rc;
     } else {
       if ((rc = make_weight_map(h, &p.w, L, pl.bn, NL))) return rc;
     }
-    // ---- output / residual views
+    // ---- output / residual pointers (the epilogue stores and loads them directly)
     if (L.kind != K_TAIL) {
       const TensorInfo& t = h->tensors[L.out];
-      const int Ht = H >> t.shift, Wt = W >> t.shift;
       void* tb = ws + P->tensor_off[L.out];
       const size_t ls = P->tensor_limb_stride[L.out];
-      if (L.kind == K_UP) {
-        for (int q = 0; q < 4; ++q)
-          if ((rc = make_act_map(h, &p.out[q], tb, ls, NL, t.channels, B, Ht, Wt, true, q >> 1, q & 1, tw, th, nb))) return rc;
-      } else {
-        if ((rc = make_act_map(h, &p.out[0], tb, ls, NL, t.channels, B, Ht, Wt, false, 0, 0, tw, th, nb))) return rc;
-        for (int q = 1; q < 4; ++q) p.out[q] = p.out[0];
-      }
       p.out_ptr = reinterpret_cast<__nv_bfloat16*>(tb);
       p.out_limb_stride = static_cast<long long>(ls / 2);
       p.out_channels = t.channels;
@@ -805,8 +722,6 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
         p.res_limb_stride = static_cast<long long>(P->tensor_limb_stride[L.res] / 2);
         p.res_channels = r.channels;
       }
-    } else {
-      for (int q = 0; q < 4; ++q) p.out[q] = p.a[0];
     }
     pl.grid = p.total_tiles < h->num_sms ? p.total_tiles : h->num_sms;
     if (pl.cluster > 1) pl.grid -= pl.grid % pl.cluster;
@@ -819,10 +734,6 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
         const char* ts = getenv("LSPG_TRACE_SKIP");
         p.trace_skip = ts ? atoi(ts) : 0;
       }
-    }
-    {
-      const char* fl = getenv("LSPG_DEBUG_FAULT_LAYER");      // test hook: see ConvParams::debug_fault
-      if (fl && atoi(fl) == static_cast<int>(P->layers.size()) && !g.patch) p.debug_fault = 1;
     }
     if (pl.split) {
       ReduceParams& r = pl.red;
@@ -892,27 +803,25 @@ int ensure_smem(K kernel, int bytes, int device, unsigned long long* done_mask) 
 
 const void* g_last_func = nullptr;     // host stub of the most recent conv launch (identifies graph nodes after capture)
 
-template <int BN, int NL, bool TAIL, bool CSP = false>
-int launch_conv(const ConvParams& p, int grid, int device, cudaStream_t st, int cluster = 1) {
-  using Cfg = ConvCfg<BN, NL, TAIL, CSP>;
+template <int BN, int NL, bool TAIL>
+int launch_conv(const ConvParams& p, int grid, int device, cudaStream_t st) {
+  using Cfg = ConvCfg<BN, NL, TAIL>;
   static unsigned long long done = 0;
-  int rc = ensure_smem(conv_umma_kernel<BN, NL, TAIL, CSP>, Cfg::kSmemBytes, device, &done);
+  int rc = ensure_smem(conv_umma_kernel<BN, NL, TAIL>, Cfg::kSmemBytes, device, &done);
   if (rc) return rc;
-  g_last_func = reinterpret_cast<const void*>(conv_umma_kernel<BN, NL, TAIL, CSP>);
-  CUDA_TRY(launch_pdl_cluster(conv_umma_kernel<BN, NL, TAIL, CSP>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, cluster, p));
+  g_last_func = reinterpret_cast<const void*>(conv_umma_kernel<BN, NL, TAIL>);
+  CUDA_TRY(launch_pdl_cluster(conv_umma_kernel<BN, NL, TAIL>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, 1, p));
   return LSPG_OK;
 }
 
-// Epilogue warps: 4 for the tail (one fp32 / uint8 scatter per pixel), 8 for every other patch / pair kernel.
-template <int BN, int NL, bool TAIL, int CL, bool CSP = false>
-int launch_patch(const ConvParams& p, int grid, int device, cudaStream_t st, int cluster = CL) {
-  using Cfg = PatchCfg<BN, NL, TAIL, CSP>;
-  constexpr int EW = TAIL ? 4 : 8;
+template <int BN, int NL, bool TAIL, int CL>
+int launch_patch(const ConvParams& p, int grid, int device, cudaStream_t st) {
+  using Cfg = PatchCfg<BN, NL, TAIL>;
   static unsigned long long done = 0;
-  int rc = ensure_smem(conv_patch_kernel<BN, NL, TAIL, CL, EW, CSP>, Cfg::kSmemBytes, device, &done);
+  int rc = ensure_smem(conv_patch_kernel<BN, NL, TAIL, CL>, Cfg::kSmemBytes, device, &done);
   if (rc) return rc;
-  g_last_func = reinterpret_cast<const void*>(conv_patch_kernel<BN, NL, TAIL, CL, EW, CSP>);
-  CUDA_TRY(launch_pdl_cluster(conv_patch_kernel<BN, NL, TAIL, CL, EW, CSP>, dim3(grid), dim3(64 + EW * 32), Cfg::kSmemBytes, st, cluster, p));
+  g_last_func = reinterpret_cast<const void*>(conv_patch_kernel<BN, NL, TAIL, CL>);
+  CUDA_TRY(launch_pdl_cluster(conv_patch_kernel<BN, NL, TAIL, CL>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, CL, p));
   return LSPG_OK;
 }
 
@@ -921,30 +830,7 @@ int launch_patch_cl(const ConvParams& p, int grid, int cluster, int device, cuda
   return cluster == 2 ? launch_patch<BN, NL, TAIL, 2>(p, grid, device, st) : launch_patch<BN, NL, TAIL, 1>(p, grid, device, st);
 }
 
-template <int BN, int NL>
-int launch_pair(const ConvParams& p, int grid, int device, cudaStream_t st) {
-  constexpr bool STK = (BN == 64 && NL == 2);          // must agree with pair_stacked()
-  using Cfg = PairCfg<BN, NL, STK>;
-  static unsigned long long done = 0;
-  int rc = ensure_smem(conv_pair_kernel<BN, NL, 8, STK>, Cfg::kSmemBytes, device, &done);
-  if (rc) return rc;
-  g_last_func = reinterpret_cast<const void*>(conv_pair_kernel<BN, NL, 8, STK>);
-  CUDA_TRY(launch_pdl_cluster(conv_pair_kernel<BN, NL, 8, STK>, dim3(grid), dim3(64 + 8 * 32), Cfg::kSmemBytes, st, 2, p));
-  return LSPG_OK;
-}
-
 int launch_layer(const PlanLayer& pl, int kind, int NL, int device, cudaStream_t st) {
-  if (pl.pair) {
-    if (pl.bn == 256) return NL == 1 ? launch_pair<256, 1>(pl.prm, pl.grid, device, st) : launch_pair<256, 2>(pl.prm, pl.grid, device, st);
-    if (pl.bn == 64) return NL == 1 ? launch_pair<64, 1>(pl.prm, pl.grid, device, st) : launch_pair<64, 2>(pl.prm, pl.grid, device, st);
-    return NL == 1 ? launch_pair<128, 1>(pl.prm, pl.grid, device, st) : launch_pair<128, 2>(pl.prm, pl.grid, device, st);
-  }
-  if (pl.csplit) {          // split-K inside a cluster of pl.csplit CTAs (one tile per CTA, grid = tiles x csplit)
-    const int cs = pl.csplit;
-    if (pl.patch) return NL == 1 ? launch_patch<64, 1, false, 1, true>(pl.prm, pl.grid, device, st, cs) : launch_patch<64, 2, false, 1, true>(pl.prm, pl.grid, device, st, cs);
-    if (pl.bn == 128) return NL == 1 ? launch_conv<128, 1, false, true>(pl.prm, pl.grid, device, st, cs) : launch_conv<128, 2, false, true>(pl.prm, pl.grid, device, st, cs);
-    return NL == 1 ? launch_conv<64, 1, false, true>(pl.prm, pl.grid, device, st, cs) : launch_conv<64, 2, false, true>(pl.prm, pl.grid, device, st, cs);
-  }
   if (pl.patch) {
     const int c = pl.cluster;
     if (kind == K_TAIL) return NL == 1 ? launch_patch_cl<16, 1, true>(pl.prm, pl.grid, c, device, st) : launch_patch_cl<16, 2, true>(pl.prm, pl.grid, c, device, st);
@@ -1114,8 +1000,8 @@ int lspg_create(lspg_handle* out, int variant, int ngf, int num_downs, int in_nc
     if (device >= count) return fail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-      return fail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_100a code only (no fallback)", device,
+    if (prop.major != 9 || prop.minor != 0)
+      return fail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device,
                   prop.major, prop.minor);
     h->num_sms = prop.multiProcessorCount;
     CUDA_TRY(cudaSetDevice(device));
@@ -1213,7 +1099,7 @@ static int forward_impl(lspg_handle h, const float* feature_map, int64_t fm_bstr
                         void* out, int out_is_u8, int batch, int height, int width, void* workspace, size_t workspace_bytes_in,
                         int mode, void* stream) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
-  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle: lspg_forward needs an sm_100 device (no CPU path exists)");
+  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle: lspg_forward needs an sm_90 device (no CPU path exists)");
   if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspg_load_weights has not been called");
   for (const auto& L : h->layers)
     if (!L.has_w)
@@ -1286,7 +1172,7 @@ int lspg_draw_feature_maps(lspg_handle h, const float* landmarks, const float* s
   if (batch <= 0 || height <= 0 || width <= 0) return fail(LSPG_EINVAL, "bad shape %d x %d x %d", batch, height, width);
   if (shoulders != nullptr && (n_shoulder_points < 0 || n_shoulder_points % 2 != 0))
     return fail(LSPG_EINVAL, "n_shoulder_points must be even (two polylines), got %d", n_shoulder_points);
-  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle: lspg_draw_feature_maps needs an sm_100 device (no CPU path exists)");
+  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle: lspg_draw_feature_maps needs an sm_90 device (no CPU path exists)");
   CUDA_TRY(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaMemsetAsync(out_fm, 0, sizeof(float) * static_cast<size_t>(batch) * height * width, st));
@@ -1380,17 +1266,14 @@ int lspg_debug_layer_geo(lspg_handle h, int layer, int batch, int height, int wi
   const Layer& L = h->layers[layer];
   const Geo g = layer_geo(h, L, batch, height, width);
   memset(o, 0, sizeof(*o));
-  o->kernel = g.pair ? 2 : (g.patch ? 1 : 0);
+  o->kernel = g.patch ? 1 : 0;
   o->bn = g.bn;
   o->tile_w = g.tw; o->tile_h = g.th; o->tile_n = g.nb;
   o->m_tiles = g.m_tiles; o->n_tiles = g.n_tiles; o->n_phases = L.n_phases;
   o->n_split = g.n_split; o->split_len = g.split_len; o->k_items = g.k_items;
   const int sms = h->num_sms_or_default();
-  int ctas = std::min(g.tiles_per_split * g.n_split, sms);
-  if (g.pair) ctas -= ctas % 2;
-  o->ctas = ctas;
+  o->ctas = std::min(g.tiles_per_split * g.n_split, sms);
   o->partial_bytes = static_cast<int64_t>(g.partial_bytes);
-  o->cluster_split = g.csplit;
   return LSPG_OK;
 }
 

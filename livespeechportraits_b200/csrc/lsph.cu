@@ -454,7 +454,7 @@ int lsph_create(lsph_handle* out, const lsph_config* c, int device) {
     if (device >= count) return hfail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
     cudaDeviceProp prop;
     HCUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return hfail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_100a code only (no fallback)", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return hfail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device, prop.major, prop.minor);
   }
   *out = h.release();
   return LSPG_OK;
@@ -606,7 +606,7 @@ int lsph_debug_packed(lsph_handle h, int which, float* dst, int64_t count) {
 int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
                   const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream) {
   if (!h) return hfail(LSPG_EINVAL, "null handle");
-  if (h->device < 0) return hfail(LSPG_ENODEV, "host-only handle: lsph_generate needs an sm_100 device (no CPU path exists)");
+  if (h->device < 0) return hfail(LSPG_ENODEV, "host-only handle: lsph_generate needs an sm_90 device (no CPU path exists)");
   if (!h->weights_loaded) return hfail(LSPG_ESTATE, "lsph_load_weights has not been called");
   const lsph_config& c = h->cfg;
   if (!audio_feats || !pre_headpose || !out_pred) return hfail(LSPG_EINVAL, "null buffer");

@@ -8,8 +8,8 @@ DataParallel ``module.`` prefix), same ``forward(input[B,13,H,W] fp32) -> [B,3,H
 optional ``DataParallel`` wrap, ``init_weights`` finds real ``Conv2d``/``BatchNorm2d`` leaves).
 
 The module tree only HOLDS parameters.  ``forward`` never runs a torch op on them: it hands device pointers
-to the C-ABI library (include/lspg.h), which runs the hand-written sm_100a kernels on the current CUDA stream.
-There is no CPU or eager fallback: a CPU input, a non-Blackwell device or a missing library raises.
+to the C-ABI library (include/lspg.h), which runs the hand-written sm_90a kernels on the current CUDA stream.
+There is no CPU or eager fallback: a CPU input, a device other than sm_90 (H100) or a missing library raises.
 """
 from __future__ import annotations
 
@@ -50,7 +50,7 @@ class Feature2Face_G(nn.Module):
         size = getattr(opt, "size", "normal")
         if size not in _lib.LSPG_VARIANT:
             raise NotImplementedError(
-                f"opt.size={size!r}: only 'normal' and 'large' are built for B200 (the 'small' U-Net takes a 23-channel "
+                f"opt.size={size!r}: only 'normal' and 'large' are built for H100 (the 'small' U-Net takes a 23-channel "
                 "input that no shipped config produces)")
         self.variant = size
         self.ngf = int(getattr(opt, "ngf", 64))
@@ -152,13 +152,13 @@ class Feature2Face_G(nn.Module):
         # parameters from the replicas (they would upload empty weights).  The reference's multi-GPU hook
         # (models/networks.py:392-401) is replaced by one process per GPU: parallel.ShardedRenderer.
         raise NotImplementedError(
-            "Feature2Face_G (B200) cannot be replicated by nn.DataParallel over several devices: the module owns a native "
+            "Feature2Face_G (H100) cannot be replicated by nn.DataParallel over several devices: the module owns a native "
             "handle per device.  Wrap it with device_ids=[one id] (what demo.py does) or shard frames over processes with "
             "livespeechportraits_b200.parallel.ShardedRenderer")
 
     def _ensure_handle(self, device: torch.device) -> None:
         if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: inputs must live on a B200 (sm_100) device")
+            raise RuntimeError("livespeechportraits_b200 has no CPU path: inputs must live on an H100 (sm_90) device")
         idx = device.index if device.index is not None else torch.cuda.current_device()
         if self._handle and self._device_index == idx:
             return

@@ -27,7 +27,7 @@ from . import _lib
 def config_from_opt(opt) -> _lib.LsphConfig:
     """The option fields Audio2Headpose.__init__ reads (models/audio2headpose.py:8-37)."""
     if getattr(opt, "feature_decoder", "WaveNet") != "WaveNet":
-        raise NotImplementedError("only the WaveNet decoder (the shipped default) is built for B200; the LSTM decoder is not autoregressive")
+        raise NotImplementedError("only the WaveNet decoder (the shipped default) is built for H100; the LSTM decoder is not autoregressive")
     g = lambda k, d: int(getattr(opt, k, d))      # noqa: E731
     cfg = _lib.LsphConfig()
     cfg.apc_hidden = g("APC_hidden_size", 512)
@@ -59,7 +59,7 @@ class HeadposeGenerator:
             device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
         device = torch.device(device)
         if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: the headpose loop needs a B200 (sm_100) device")
+            raise RuntimeError("livespeechportraits_b200 has no CPU path: the headpose loop needs an H100 (sm_90) device")
         self.device = device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
         _lib.check_h(self._lib.lsph_create(C.byref(self._handle), C.byref(self.cfg), self.device.index))
         rf = C.c_int()
@@ -141,7 +141,7 @@ def generate_sequences(self, audio_feats, pre_headpose, fill_zero=True, sigma_sc
     """Replacement for ``Audio2HeadposeModel.generate_sequences`` (models/audio2headpose_model.py:133-187), bound to the
     reference model by ``install()``.  Same arguments, same return value ([nframe, A2H_GMM_ndim] float64 numpy)."""
     if getattr(opt, "feature_decoder", "WaveNet") != "WaveNet":
-        raise NotImplementedError("B200 headpose loop: WaveNet decoder only")
+        raise NotImplementedError("H100 headpose loop: WaveNet decoder only")
     if not fill_zero:
         return None                                                                    # audio2headpose_model.py:161-162
     net = self.Audio2Headpose.module if hasattr(self.Audio2Headpose, "module") else self.Audio2Headpose

@@ -2,7 +2,7 @@
 
 The reference's only multi-GPU hook is ``nn.DataParallel`` (models/networks.py:392-401), single process, with a
 gather of the outputs on device 0.  Frames are independent (eval-mode BatchNorm, no temporal state:
-demo.py:260-266), so the B200 layout is: contiguous block partition of the clip's frames over the ranks, no
+demo.py:260-266), so the layout is: contiguous block partition of the clip's frames over the ranks, no
 data-path collective while rendering, and ONE exchange step - every rank ends up with every frame (the
 all-gather BASELINE.json names).
 

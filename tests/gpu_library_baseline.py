@@ -1,5 +1,5 @@
 """GPU *library* baseline (not a product path): the oracle restatement executed by PyTorch eager + cuDNN on the
-same B200 - what the unmodified reference module would run (base_model.py:46-47 sets cudnn.benchmark) - in
+same H100 - what the unmodified reference module would run (base_model.py:46-47 sets cudnn.benchmark) - in
 fp32, TF32 and bf16-autocast/channels_last.  Prints frames/s so the hand-written kernels can be put beside it."""
 import os
 import sys

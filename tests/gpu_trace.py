@@ -1,4 +1,4 @@
-"""Dump the in-kernel clock64 trace of conv layers (debug tool; see conv_umma.cuh kTraceSlots).
+"""Dump the in-kernel clock64 trace of conv layers (debug tool; see conv_wgmma.cuh kTraceSlots).
     LSPG_TRACE_LAYERS=<i,j,...> [LSPG_TRACE_SKIP=<first local tile>] python tests/gpu_trace.py <variant> <mode> <B>
 One process, one generator instance per traced layer (the trace target is fixed when the launch plan is built)."""
 import os
@@ -57,9 +57,9 @@ for layer in layers:
             if not s.any():
                 break
             rel = [int(v - t0) if v else -1 for v in s]
-            print(f"   tile {i}: mma_start {rel[0]:7d} first_A {rel[1]:7d} mma_issued {rel[2]:7d} | epi_wait {rel[3]:7d} acc_ready {rel[4]:7d} "
-                  f"epi_done {rel[5]:7d} | prod_first {rel[6]:7d} prod_last {rel[7]:7d}")
-    spans = {"mma": [], "epi": [], "wait_acc": [], "total": []}
+            print(f"   tile {i}: start {rel[0]:7d} first_stage {rel[1]:7d} mma_done {rel[2]:7d} epi_done {rel[3]:7d} "
+                  f"| prod_first {rel[6]:7d} prod_last {rel[7]:7d}")
+    spans = {"wait_first_stage": [], "mma": [], "epi": [], "total": []}
     for cta in range(256):
         e = t[cta]
         if e[0] == 0:
@@ -69,11 +69,10 @@ for layer in layers:
             s = e[4 + 8 * i: 12 + 8 * i]
             if s[3] == 0:
                 break
-            if s[0]:
-                spans["mma"].append(int(s[2] - s[0]))
-            spans["epi"].append(int(s[5] - s[4]))
-            spans["wait_acc"].append(int(s[4] - s[3]))
-            last = max(last, int(s[5] - e[0]))
+            spans["wait_first_stage"].append(int(s[1] - s[0]))
+            spans["mma"].append(int(s[2] - s[1]))
+            spans["epi"].append(int(s[3] - s[2]))
+            last = max(last, int(s[3] - e[0]))
         spans["total"].append(last)
     for k, v in spans.items():
         if v:

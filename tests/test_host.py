@@ -182,7 +182,7 @@ def test_drop_in_through_the_reference_model_class(tmp_path):
 
 
 def test_tile_decode_division_by_multiply_high_is_exact():
-    """decode_tile divides tile indices by launch-time constants with multiply-high + shift (csrc/conv_umma.cuh fast_div)."""
+    """decode_tile divides tile indices by launch-time constants with multiply-high + shift (csrc/conv_wgmma.cuh fast_div)."""
     import random
     lib = _lib.load()
     rng = random.Random(0)
@@ -222,51 +222,24 @@ def _geo_table(variant, batch, height=512, width=512):
 def test_planner_invariants(variant, batch):
     """The launch planner (layer_geo in csrc/lspg.cu) on the host: tile shapes, kernel choice, split-K and wave rules."""
     table, ws = _geo_table(variant, batch)
-    sms = 148
+    sms = 132                                                              # H100 SXM (host-only handle default)
     for info, g in table:
-        assert g.tile_w * g.tile_h * g.tile_n == 128                       # one UMMA M tile
-        assert g.bn in (16, 64, 128, 256) and info.cout_pad % g.bn == 0 and g.n_tiles == info.cout_pad // g.bn
+        assert g.tile_w * g.tile_h * g.tile_n == 128                       # one M tile (two wgmma M=64 halves)
+        assert g.bn in (16, 64, 128) and info.cout_pad % g.bn == 0 and g.n_tiles == info.cout_pad // g.bn
         tiles = g.m_tiles * g.n_tiles * g.n_phases
-        if g.kernel == 2:                                                    # cta_group::2: pairs of neighbouring M tiles
-            assert g.m_tiles % 2 == 0 and g.n_split == 1 and g.ctas % 2 == 0 and (g.tile_w, g.tile_h) == (8, 16)
-        if g.kernel in (1, 2):
-            assert info.kind != 2                                            # stride-2 convs use the per-tap kernel
+        assert g.kernel in (0, 1)
+        if g.kernel == 1:
+            assert info.kind != 2 and (g.tile_w, g.tile_h) == (8, 16)      # stride-2 convs use the per-tap kernel
         if g.n_split > 1:
-            assert g.kernel != 2
             assert tiles * g.n_split <= sms                                  # split-K never spills into a second wave
             assert (g.n_split - 1) * g.split_len < g.k_items <= g.n_split * g.split_len   # every split has work
-            if g.cluster_split:
-                # the splits of a tile are one thread-block cluster (DSMEM reduction): portable cluster size, one CTA per
-                # (tile, split), nothing in the global scratch, no finisher launch
-                assert g.cluster_split == g.n_split and g.n_split in (2, 4, 8)
-                assert g.ctas == tiles * g.n_split and g.partial_bytes == 0
-                assert g.bn in (64, 128) and info.kind != 4
-            else:
-                assert g.partial_bytes == g.n_split * tiles * 128 * g.bn * 4
+            assert g.partial_bytes == g.n_split * tiles * 128 * g.bn * 4     # fp32 partials for the finisher kernel
         else:
-            assert g.partial_bytes == 0 and g.cluster_split == 0
+            assert g.partial_bytes == 0
         assert 1 <= g.ctas <= sms
     assert ws > max(g.partial_bytes for _, g in table)
     n_split_layers = sum(1 for _, g in table if g.n_split > 1)
-    n_cluster = sum(1 for _, g in table if g.cluster_split)
-    if batch >= 8:
-        assert n_split_layers >= 10 and n_cluster == n_split_layers       # from 8 frames up every split layer reduces inside its cluster
-    else:
-        assert n_cluster == 0 and (batch != 1 or n_split_layers >= 40)     # below that (measured slower) the finisher kernel stays
-
-
-def test_planner_picks_the_n_tile_with_fewer_waves():
-    def bn_of(batch, cout, hw):
-        table, _ = _geo_table("large", batch)
-        return {g.bn for info, g in table if info.kind == 1 and info.cout == cout and g.kernel == 2
-                and g.m_tiles == batch * (hw // 8) * (hw // 16)}
-    # 256 -> 256 @64^2, 16 frames: 256 pairs of N=256 tiles = 4 waves of 74 clusters; 512 pairs of N=128 = 7 half-size waves
-    assert bn_of(16, 256, 64) == {128}
-    assert bn_of(32, 256, 64) == {256}        # 7 waves vs 14 half-size waves: tie -> the wider tile
-    assert bn_of(16, 512, 32) == {256}        # 2 vs 4 half-size: tie
-    assert bn_of(32, 512, 32) == {128}        # 4 vs 7 half-size
-    # the 64-channel layers always take the resident-weights N=64 pair kernel
-    assert bn_of(16, 64, 256) == {64}
+    assert n_split_layers >= 10 and (batch != 1 or n_split_layers >= 40)
 
 
 @pytest.mark.parametrize("variant", ["normal", "large"])
@@ -335,7 +308,7 @@ def test_package_exports_public_names():
 
 def test_planner_invariants_over_random_problem_sizes():
     """Property test of layer_geo / workspace sizing through the C ABI (host only): any accepted (batch, H, W) gives tiles
-    that cover every level, split-K that stays inside one wave with non-empty K ranges, cluster splits of portable size, and a
+    that cover every level, split-K that stays inside one wave with non-empty K ranges and finisher partials sized to match, and a
     workspace at least as large as the activations + the largest partial buffer."""
     from hypothesis import given, settings, strategies as st
     lib = _lib.load()
@@ -367,13 +340,11 @@ def test_planner_invariants_over_random_problem_sizes():
             assert lib.lspg_debug_layer_geo(h, i, batch, hh, ww, C.byref(g)) == 0
             assert g.tile_w * g.tile_h * g.tile_n == 128 and g.m_tiles >= 1 and g.n_tiles >= 1
             tiles = g.m_tiles * g.n_tiles * g.n_phases
-            assert 1 <= g.ctas <= 148
+            assert 1 <= g.ctas <= 132
             if g.n_split > 1:
-                assert tiles * g.n_split <= 148 and (g.n_split - 1) * g.split_len < g.k_items <= g.n_split * g.split_len
-                assert g.cluster_split in (0, 2, 4, 8) and (g.cluster_split == 0 or g.cluster_split == g.n_split)
-                assert (g.cluster_split != 0) == (batch >= 8) or g.partial_bytes > 0
-            if g.kernel == 2:
-                assert g.m_tiles % 2 == 0 and g.ctas % 2 == 0 and g.n_split == 1
+                assert tiles * g.n_split <= 132 and (g.n_split - 1) * g.split_len < g.k_items <= g.n_split * g.split_len
+                assert g.partial_bytes == g.n_split * tiles * 128 * g.bn * 4
+            assert g.kernel in (0, 1)
             worst_partial = max(worst_partial, g.partial_bytes)
         assert need.value >= act + worst_partial
 
