@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/lspg.h.  Plain pointers and sizes only."""
+"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h and include/lspm.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
 import ctypes as C
@@ -22,6 +22,10 @@ SYMBOLS = [
 # include/lsph.h (Audio2Headpose generation loop)
 SYMBOLS_H = ["lsph_create", "lsph_load_weights", "lsph_generate", "lsph_receptive_field", "lsph_debug_packed", "lsph_destroy",
              "lsph_last_error"]
+
+# include/lspm.h (APC manifold projection: KNN + LLE)
+SYMBOLS_M = ["lspm_create", "lspm_load_database", "lspm_workspace_bytes", "lspm_knn", "lspm_project", "lspm_destroy",
+             "lspm_last_error"]
 
 
 class LsphConfig(C.Structure):
@@ -124,6 +128,18 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     for name in SYMBOLS_H:
         if name != "lsph_last_error":
             getattr(lib, name).restype = C.c_int
+    lib.lspm_last_error.restype = C.c_char_p
+    lib.lspm_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int]
+    lib.lspm_load_database.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
+    lib.lspm_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
+    lib.lspm_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                             C.c_void_p]
+    lib.lspm_project.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
+                                 C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.lspm_destroy.argtypes = [C.c_void_p]
+    for name in SYMBOLS_M:
+        if name != "lspm_last_error":
+            getattr(lib, name).restype = C.c_int
     _LIB = lib
     return lib
 
@@ -136,3 +152,8 @@ def check(code: int) -> None:
 def check_h(code: int) -> None:
     if code != 0:
         raise LspgError(code, (load().lsph_last_error() or b"").decode("utf-8", "replace"))
+
+
+def check_m(code: int) -> None:
+    if code != 0:
+        raise LspgError(code, (load().lspm_last_error() or b"").decode("utf-8", "replace"))
