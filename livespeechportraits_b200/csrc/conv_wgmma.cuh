@@ -13,11 +13,12 @@
 //     stored with stride 2 in x and y, and torch.cat([skip, deeper]) is two K ranges fed from two tensor maps -
 //     so upsample, concat, padding and stride never touch HBM as separate passes.
 //   * B tiles come from a packed weight tensor [phase*limb][Cout][K] (K-major), same 128B-swizzled layout.
-//   * Warp specialisation: warpgroup 0 = TMA producer (one warp), warpgroups 1 and 2 = consumers.  Consumer w issues
-//     wgmma.m64nBNk16 on rows [64w, 64w+64) of the tile with fp32 accumulators in registers, then runs the epilogue
-//     from those registers: folded eval-BatchNorm scale/shift in fp32, residual, ReLU, 16-bit (hi, lo) NHWC stores.
-//     The producer keeps filling the ring for the next tile while the consumers finish the current one.  The tail
-//     variant applies tanh and scatters fp32 NCHW or uint8 HWC directly.
+//   * Warp specialisation: warpgroup 0 = TMA producer (one warp), warpgroups 1 and 2 = consumers issuing
+//     wgmma.m64nBNk16 with fp32 accumulators in registers, then running the epilogue from those registers: folded
+//     eval-BatchNorm scale/shift in fp32, residual, ReLU, 16-bit (hi, lo) NHWC stores.  The tail variant applies tanh
+//     and scatters fp32 NCHW or uint8 HWC directly.
+//     conv_umma_kernel: consumer w owns rows [64w, 64w+64) of every tile.  conv_patch_kernel: ping-pong, consumer w
+//     owns every other tile (all 128 rows, two accumulators), so its epilogue runs under the other one's MMAs.
 //   * NL = 2 ("parity" precision): activations and weights are split into fp16 hi + lo limbs; each K step issues
 //     hi*hi + hi*lo + lo*hi into one accumulator (22 mantissa bits per operand, fp32 accumulate) and the epilogue writes
 //     both limbs.  NL = 1 ("fast"): one bf16 limb, one MMA per K step.
@@ -107,12 +108,14 @@ struct alignas(64) ConvParams {
   CUtensorMap w;             // packed weights, dims {K, Cout_pad, limb*n_phases + phase} (patch kernel: {kc, Cout, tap, limb*phase})
 };
 
-// Shared-memory regions after the operand rings: barriers, then (tail) the accumulator staging of the tail epilogue.
+// Shared-memory regions after the operand rings: barriers, then (tail) the accumulator staging of the tail epilogue,
+// kTailRows rows (one tile for the per-tap kernel, whose consumers split every tile; one tile per consumer warpgroup
+// for the patch kernel, whose consumers own whole tiles).
 constexpr int kBarBytes = 1024;
 constexpr int kTailStride = 17;                                      // floats per staged tail row (16 + 1: no bank conflicts)
-template <bool TAIL>
+template <bool TAIL, int kTailRows = kTileM>
 struct AuxCfg {
-  static constexpr int kTailBytes = TAIL ? kTileM * kTailStride * 4 : 0;
+  static constexpr int kTailBytes = TAIL ? kTailRows * kTailStride * 4 : 0;
   static constexpr int kBytes = kBarBytes + kTailBytes;
 };
 
@@ -131,7 +134,9 @@ struct ConvCfg {
 
 // Debug trace layout per CTA: [0] kernel entry, [1] prologue done, [2]/[3] globaltimer (ns) at entry/exit, then per
 // local tile i (up to kTraceTiles): base = 4 + 8*i: +0 consumers start the tile, +1 first stage landed, +2 last MMA
-// retired, +3 epilogue done, +6 PROD first load of the tile issued, +7 PROD last load issued
+// retired, +3 epilogue done, +6 PROD first load of the tile issued, +7 PROD last load issued.  +0..+3 are written by
+// the leader thread of the warpgroup that runs the tile's MMAs (the patch kernel: the tile's owner, +0 once the
+// other warpgroup has issued the previous tile; the per-tap kernel: warpgroup 1).
 constexpr int kTraceTiles = 12;
 constexpr int kTraceSlots = 4 + 8 * kTraceTiles + 4;   // tail: [+0] clock64 at kernel exit
 
@@ -216,33 +221,34 @@ __device__ __forceinline__ void row_pixel(const ConvParams& p, const TileCoord& 
   n = tc.n0 + (row >> (p.tw_log2 + p.th_log2));
 }
 
-// Consumer epilogue of one tile, straight from the wgmma accumulator registers of warpgroup `cw` (rows [64cw, 64cw+64)).
+// Consumer epilogue of the 64 tile rows [rb, rb+64) held by one m64nBN accumulator of the calling warpgroup.
 // Thread layout of the m64nBN accumulator: rows r0 = 16*warp + lane/4 and r0 + 8, columns 8j + 2*(lane%4) and +1
 // (d[4j], d[4j+1] for r0; d[4j+2], d[4j+3] for r0 + 8).
 // Modes: split-K partial (fp32 rows to the global scratch), tail (via shared memory: tanh and
 // the NCHW / uint8 scatter want all 12 columns of a pixel in one thread), and the regular epilogue.
+// Tail only: `tail_stg` is this call's 64-row staging region, `tail_bar` the calling warpgroup's named barrier.
 template <int BN, int NL, bool TAIL>
-__device__ __forceinline__ void epilogue_regs(const ConvParams& p, const float (&acc)[BN / 2], const TileCoord& tc, int t, int cw,
-                                              float* tail_stg) {
+__device__ __forceinline__ void epilogue_regs(const ConvParams& p, const float (&acc)[BN / 2], const TileCoord& tc, int t, int rb,
+                                              float* tail_stg, int tail_bar) {
   const int wtid = threadIdx.x & 127;
   const int warp = wtid >> 5, lane = wtid & 31;
-  const int r0 = cw * 64 + warp * 16 + (lane >> 2);
+  const int r0 = rb + warp * 16 + (lane >> 2);
   const int c0 = 2 * (lane & 3);
   if constexpr (TAIL) {
     // ---- tail: 16 columns = 4 phases x 3 channels (+4 pad); tanh; fp32 NCHW scatter or fused tensor2im
-    float* stg = tail_stg + cw * 64 * kTailStride;
-    ptx::named_bar_sync(1 + cw, 128);                     // the previous tile's rows have been read
+    float* stg = tail_stg;
+    ptx::named_bar_sync(tail_bar, 128);                   // the previous tile's rows have been read
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float* s = stg + (r0 - cw * 64 + 8 * h) * kTailStride + 8 * j + c0;
+        float* s = stg + (r0 - rb + 8 * h) * kTailStride + 8 * j + c0;
         s[0] = acc[4 * j + 2 * h];
         s[1] = acc[4 * j + 2 * h + 1];
       }
-    ptx::named_bar_sync(1 + cw, 128);
+    ptx::named_bar_sync(tail_bar, 128);
     if (wtid >= 64) return;
-    const int row = cw * 64 + wtid;
+    const int row = rb + wtid;
     const float* v = stg + wtid * kTailStride;
     int pn, py_, px_;
     row_pixel(p, tc, row, pn, py_, px_);
@@ -342,7 +348,7 @@ __device__ __forceinline__ void epilogue_regs(const ConvParams& p, const float (
   }
 }
 
-// Release of a consumed ring stage: one arrive per consumer warpgroup on the stage's empty barrier in every CTA of `CL`
+// Release of a consumed ring stage: one arrive per consuming warpgroup on the stage's empty barrier in every CTA of `CL`
 // (a stage filled by multicast is refilled only after every CTA that received it is done with it).
 template <int CL>
 __device__ __forceinline__ void release_stage(uint64_t* bar) {
@@ -490,7 +496,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_umma_kernel(const __grid_con
       ptx::wgmma_wait<0>();
       if (prev >= 0 && wg_leader) release_stage<1>(&empty_bar[prev]);
       if (threadIdx.x == 128) trace_tile(p, lt, 2);
-      epilogue_regs<BN, NL, TAIL>(p, acc, tc, t, cw, tail_stg);
+      epilogue_regs<BN, NL, TAIL>(p, acc, tc, t, 64 * cw, tail_stg + cw * 64 * kTailStride, 1 + cw);
       if (threadIdx.x == 128) trace_tile(p, lt, 3);
     }
   }
@@ -504,17 +510,25 @@ __global__ void __launch_bounds__(kThreads, 1) conv_umma_kernel(const __grid_con
 // addressed inside it: with TW = 8 an 8-row core-matrix group of the wgmma A operand is one image row of the patch, so
 // the shifted A tile of tap (dx,dy) is the same swizzled buffer described by
 //   start = patch + ((dy-dy0)*PW + (dx-dx0)) * 128 B,   stride between 8-row groups (SBO) = PW * 128 B,
-// and consumer warpgroup w starts 8 image rows further down (rows 64w.. of the 8x16 tile).
+// and tile rows 64..127 (the second m64 MMA) start 8 image rows further down.
 // The swizzle phase of a row is a function of its absolute smem address for both TMA and the tensor core, so rows that
 // TMA wrote are read back consistently at any 128-byte-aligned start (descriptor base offset 0).
 // A and B move through separate mbarrier rings: an A patch is consumed by n_taps B tiles.
+// The consumers ping-pong: warpgroup 1 owns the CTA's even local tiles and warpgroup 2 the odd ones, all 128 rows of
+// each (two m64nBN accumulators), so one warpgroup runs its epilogue while the other issues the next tile's MMAs.
 // ====================================================================================================
 constexpr int kPatchSlot = 23 * 1024;           // >= 10*18*128 = 23040 bytes
 constexpr int kPatchStride = 23 * 1024;         // distance between patch buffers (1024-byte aligned)
 
+// Register split of the patch kernel (setmaxnreg): the launch gives every thread 168 registers (384 threads, one CTA per
+// SM); the producer warpgroup gives most of its share to the consumers, which hold 2 x BN/2 accumulator floats each.
+constexpr int kProducerRegs = 40;
+constexpr int kConsumerRegs = 232;
+static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file of one SM");
+
 template <int BN, int NL, bool TAIL>
 struct PatchCfg {
-  using Aux = AuxCfg<TAIL>;
+  using Aux = AuxCfg<TAIL, 2 * kTileM>;
   static constexpr int kBTile = BN * 128;
   // taps per B stage: each stage costs one barrier round trip, so a stage must carry enough tensor work: 2 taps for
   // N=128 bf16, 2-3 for N=64, all 9 for the tail.
@@ -548,6 +562,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
   uint64_t* aempty_bar = afull_bar + Cfg::kAStages;         // [kAStages]
   uint64_t* bfull_bar = aempty_bar + Cfg::kAStages;         // [kBStages]
   uint64_t* bempty_bar = bfull_bar + Cfg::kBStages;         // [kBStages]
+  uint64_t* turn_bar = bempty_bar + Cfg::kBStages;          // [2]: consumer warpgroup w has issued every MMA of a tile
   float* tail_stg = reinterpret_cast<float*>(aux + kBarBytes);
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // provably warp-uniform
@@ -557,8 +572,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
   if (warp == 0 && lane == 0) {
     for (int i = 0; i < 4; ++i) ptx::prefetch_tmap(&p.a[i]);
     ptx::prefetch_tmap(&p.w);
-    for (int i = 0; i < Cfg::kAStages; ++i) { ptx::mbar_init(&afull_bar[i], 1); ptx::mbar_init(&aempty_bar[i], 2); }
-    for (int i = 0; i < Cfg::kBStages; ++i) { ptx::mbar_init(&bfull_bar[i], 1); ptx::mbar_init(&bempty_bar[i], 2 * CL); }
+    // every stage is consumed by the one warpgroup that owns its tile (in each CTA of the cluster for B)
+    for (int i = 0; i < Cfg::kAStages; ++i) { ptx::mbar_init(&afull_bar[i], 1); ptx::mbar_init(&aempty_bar[i], 1); }
+    for (int i = 0; i < Cfg::kBStages; ++i) { ptx::mbar_init(&bfull_bar[i], 1); ptx::mbar_init(&bempty_bar[i], CL); }
+    for (int i = 0; i < 2; ++i) ptx::mbar_init(&turn_bar[i], 1);
     ptx::fence_mbar_init();
   }
   __syncthreads();
@@ -573,126 +590,160 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
   const int patch_bytes = p.patch_w * p.patch_h * 128;
   const int n_groups = (p.n_taps + Cfg::kTPS - 1) / Cfg::kTPS;
 
-  if (warp == 0) {
-    // ===================================================================== TMA producer
-    // Flat sequence of items (tile, concat-chunk ci).  The A patch of item j+1 is issued in the middle of item
-    // j's B tiles so that it is in flight while the consumers still work on item j.
-    ptx::pdl_wait();                // activations are written by the previous kernel
-    int ia = 0, ib = 0;
-    uint32_t pha = 0, phb = 0;
-    int a_tile = t0, a_ci = -1;            // cursor of the next A patch to issue (-1: take the tile's first item)
-    auto issue_a = [&]() {
-      if (a_tile >= p.total_tiles) return;
-      const TileCoord tc = decode_tile(p, a_tile);
-      const int ci0 = tc.split * p.split_len;
-      const int ci1 = (ci0 + p.split_len < kb_per_tap) ? ci0 + p.split_len : kb_per_tap;
-      if (a_ci < 0) a_ci = ci0;
-      const int s = (a_ci < p.chunks[0]) ? 0 : 1;
-      const int c = (s == 0) ? a_ci : a_ci - p.chunks[0];
-      ptx::mbar_wait(&aempty_bar[ia], pha ^ 1);
-      if (ptx::elect_one()) {
-        ptx::mbar_expect_tx(&afull_bar[ia], NL * patch_bytes);
+  if (warp < 4) {
+    ptx::setmaxnreg_dec<kProducerRegs>();   // the whole warpgroup; warps 1-3 have no further work
+    if (warp == 0) {
+      // ===================================================================== TMA producer
+      // Flat sequence of items (tile, concat-chunk ci).  The A patch of item j+1 is issued in the middle of item
+      // j's B tiles so that it is in flight while the consumers still work on item j.
+      ptx::pdl_wait();                // activations are written by the previous kernel
+      int ia = 0, ib = 0;
+      uint32_t pha = 0, phb = 0;
+      int a_tile = t0, a_ci = -1;            // cursor of the next A patch to issue (-1: take the tile's first item)
+      auto issue_a = [&]() {
+        if (a_tile >= p.total_tiles) return;
+        const TileCoord tc = decode_tile(p, a_tile);
+        const int ci0 = tc.split * p.split_len;
+        const int ci1 = (ci0 + p.split_len < kb_per_tap) ? ci0 + p.split_len : kb_per_tap;
+        if (a_ci < 0) a_ci = ci0;
+        const int s = (a_ci < p.chunks[0]) ? 0 : 1;
+        const int c = (s == 0) ? a_ci : a_ci - p.chunks[0];
+        ptx::mbar_wait(&aempty_bar[ia], pha ^ 1);
+        if (ptx::elect_one()) {
+          ptx::mbar_expect_tx(&afull_bar[ia], NL * patch_bytes);
 #pragma unroll
-        for (int l = 0; l < NL; ++l)
-          ptx::tma_load_5d(&p.a[s], &afull_bar[ia], a_ring + ia * Cfg::kAStage + l * kPatchStride, c * kChunk,
-                           tc.x0 + p.patch_dx0[tc.z], tc.y0 + p.patch_dy0[tc.z], tc.n0, l);
-      }
-      __syncwarp();
-      if (++ia == Cfg::kAStages) { ia = 0; pha ^= 1; }
-      if (++a_ci == ci1) { a_ci = -1; a_tile += tstep; }
-    };
-    issue_a();
-    const int a_after_group = (n_groups > 1) ? 1 : 0;
-    int lt = 0;
-    for (int t = t0; t < p.total_tiles; t += tstep, ++lt) {
-      const TileCoord tc = decode_tile(p, t);
-      const int ci0 = tc.split * p.split_len;
-      const int ci1 = (ci0 + p.split_len < kb_per_tap) ? ci0 + p.split_len : kb_per_tap;
-      if (lane == 0) trace_tile(p, lt, 6);
-      for (int ci = ci0; ci < ci1; ++ci) {
-        for (int g = 0; g < n_groups; ++g) {
-          ptx::mbar_wait(&bempty_bar[ib], phb ^ 1);
-          if (ptx::elect_one()) {
-            uint8_t* st = b_ring + ib * Cfg::kBStage;
-            if constexpr (CL == 1 && NL == 1) {
-              ptx::mbar_expect_tx(&bfull_bar[ib], Cfg::kBStage);
-              // one box = kTPS taps x BN rows x 64 channels (taps beyond n_taps are zero-filled)
-              ptx::tma_load_4d(&p.w, &bfull_bar[ib], st, ci * kChunk, tc.nt * BN, g * Cfg::kTPS, tc.z);
-            } else {
-              // per-tap boxes of BN/CL rows.  Stage layout [tap][limb][BN rows].  With CL = 2 this CTA fetches rows
-              // [crank*BN/CL, +BN/CL) of every tile and multicasts them to the whole cluster.
-              const int tap0 = g * Cfg::kTPS;
-              const int ntap = (tap0 + Cfg::kTPS < p.n_taps) ? Cfg::kTPS : p.n_taps - tap0;
-              ptx::mbar_expect_tx(&bfull_bar[ib], NL * ntap * Cfg::kBTile);
-              constexpr int kRows = BN / CL;
-              for (int ti = 0; ti < ntap; ++ti)
-#pragma unroll
-                for (int l = 0; l < NL; ++l) {
-                  uint8_t* dst = st + (ti * NL + l) * Cfg::kBTile + crank * kRows * 128;
-                  if constexpr (CL == 1)
-                    ptx::tma_load_4d(&p.w, &bfull_bar[ib], dst, ci * kChunk, tc.nt * BN, tap0 + ti, l * p.n_phases + tc.z);
-                  else
-                    ptx::tma_load_4d_mc(&p.w, &bfull_bar[ib], dst, ci * kChunk, tc.nt * BN + crank * kRows, tap0 + ti,
-                                        l * p.n_phases + tc.z, kMask);
-                }
-            }
-          }
-          __syncwarp();
-          if (++ib == Cfg::kBStages) { ib = 0; phb ^= 1; }
-          if (g == a_after_group) issue_a();
+          for (int l = 0; l < NL; ++l)
+            ptx::tma_load_5d(&p.a[s], &afull_bar[ia], a_ring + ia * Cfg::kAStage + l * kPatchStride, c * kChunk,
+                             tc.x0 + p.patch_dx0[tc.z], tc.y0 + p.patch_dy0[tc.z], tc.n0, l);
         }
+        __syncwarp();
+        if (++ia == Cfg::kAStages) { ia = 0; pha ^= 1; }
+        if (++a_ci == ci1) { a_ci = -1; a_tile += tstep; }
+      };
+      issue_a();
+      const int a_after_group = (n_groups > 1) ? 1 : 0;
+      int lt = 0;
+      for (int t = t0; t < p.total_tiles; t += tstep, ++lt) {
+        const TileCoord tc = decode_tile(p, t);
+        const int ci0 = tc.split * p.split_len;
+        const int ci1 = (ci0 + p.split_len < kb_per_tap) ? ci0 + p.split_len : kb_per_tap;
+        if (lane == 0) trace_tile(p, lt, 6);
+        for (int ci = ci0; ci < ci1; ++ci) {
+          for (int g = 0; g < n_groups; ++g) {
+            ptx::mbar_wait(&bempty_bar[ib], phb ^ 1);
+            if (ptx::elect_one()) {
+              uint8_t* st = b_ring + ib * Cfg::kBStage;
+              if constexpr (CL == 1 && NL == 1) {
+                ptx::mbar_expect_tx(&bfull_bar[ib], Cfg::kBStage);
+                // one box = kTPS taps x BN rows x 64 channels (taps beyond n_taps are zero-filled)
+                ptx::tma_load_4d(&p.w, &bfull_bar[ib], st, ci * kChunk, tc.nt * BN, g * Cfg::kTPS, tc.z);
+              } else {
+                // per-tap boxes of BN/CL rows.  Stage layout [tap][limb][BN rows].  With CL = 2 this CTA fetches rows
+                // [crank*BN/CL, +BN/CL) of every tile and multicasts them to the whole cluster.
+                const int tap0 = g * Cfg::kTPS;
+                const int ntap = (tap0 + Cfg::kTPS < p.n_taps) ? Cfg::kTPS : p.n_taps - tap0;
+                ptx::mbar_expect_tx(&bfull_bar[ib], NL * ntap * Cfg::kBTile);
+                constexpr int kRows = BN / CL;
+                for (int ti = 0; ti < ntap; ++ti)
+#pragma unroll
+                  for (int l = 0; l < NL; ++l) {
+                    uint8_t* dst = st + (ti * NL + l) * Cfg::kBTile + crank * kRows * 128;
+                    if constexpr (CL == 1)
+                      ptx::tma_load_4d(&p.w, &bfull_bar[ib], dst, ci * kChunk, tc.nt * BN, tap0 + ti, l * p.n_phases + tc.z);
+                    else
+                      ptx::tma_load_4d_mc(&p.w, &bfull_bar[ib], dst, ci * kChunk, tc.nt * BN + crank * kRows, tap0 + ti,
+                                          l * p.n_phases + tc.z, kMask);
+                  }
+              }
+            }
+            __syncwarp();
+            if (++ib == Cfg::kBStages) { ib = 0; phb ^= 1; }
+            if (g == a_after_group) issue_a();
+          }
+        }
+        if (lane == 0) trace_tile(p, lt, 7);
       }
-      if (lane == 0) trace_tile(p, lt, 7);
     }
-  } else if (warp >= 4) {
+  } else {
+    ptx::setmaxnreg_inc<kConsumerRegs>();
     // ===================================================================== consumers (warpgroups 1, 2)
+    // Ping-pong: warpgroup w owns the local tiles lt with lt % 2 == w, all 128 rows (acc[0]: rows 0-63, acc[1]: rows
+    // 64-127, read 8 image rows further down the patch).  Every accumulator element sees the same operands in the same
+    // K order as one m64 half of a tile split across both warpgroups would.  A ring stage is consumed by the warpgroup
+    // that owns its tile; the other one moves its cursors past the tile's stages.
+    // MMA issue alternates by tile: tile lt > 0 starts once the other warpgroup has issued every MMA of tile lt-1
+    // (turn_bar), so the tensor pipe finishes one tile before it starts the next and the owner's epilogue runs under the
+    // next tile's MMAs.  This cannot deadlock: issuing tile lt-1 needs only the stages of tile lt-1, which the producer
+    // fills in tile order into slots freed by tiles <= lt-2, and the waiting warpgroup released every stage of its own
+    // tile lt-2 before its epilogue.  Each wait depends on an event of an earlier tile only.
     ptx::pdl_wait();   // residual reads, output / split-K partial writes must not overtake the previous kernel
-    const int cw = (warp >> 2) - 1;
+    const int wg = (warp >> 2) - 1;
     const bool wg_leader = (threadIdx.x & 127) == 0;
     int ia = 0, ib = 0;
     uint32_t pha = 0, phb = 0;
     const uint32_t sbo = static_cast<uint32_t>(p.patch_w) * 128u;
-    const uint32_t row_off = static_cast<uint32_t>(cw * 8 * p.patch_w) * 128u;   // 8 image rows down for warpgroup 1
+    const uint32_t row_off = static_cast<uint32_t>(8 * p.patch_w) * 128u;   // tile rows 64..127: 8 image rows down
     const bool boff = p.desc_base_offset != 0;
+    float* stg = tail_stg + wg * kTileM * kTailStride;                       // this warpgroup's tail staging (128 rows)
     int lt = 0;
     for (int t = t0; t < p.total_tiles; t += tstep, ++lt) {
       const TileCoord tc = decode_tile(p, t);
       const int ci0 = tc.split * p.split_len;
       const int ci1 = (ci0 + p.split_len < kb_per_tap) ? ci0 + p.split_len : kb_per_tap;
-      if (threadIdx.x == 128) trace_tile(p, lt, 0);
-      float acc[BN / 2];
+      if ((lt & 1) != wg) {
+        // the other warpgroup's tile: (ci1 - ci0) A patches and n_groups B stages per patch
+        ia += ci1 - ci0;
+        pha ^= static_cast<uint32_t>(ia / Cfg::kAStages) & 1u;
+        ia %= Cfg::kAStages;
+        ib += (ci1 - ci0) * n_groups;
+        phb ^= static_cast<uint32_t>(ib / Cfg::kBStages) & 1u;
+        ib %= Cfg::kBStages;
+        continue;
+      }
+      if (lt > 0) ptx::mbar_wait(&turn_bar[wg ^ 1], static_cast<uint32_t>((lt - 1) >> 1) & 1u);
+      if (wg_leader) trace_tile(p, lt, 0);
+      float acc[2][BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.0f;
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.0f;
       // the stage consumed one step earlier is released once the MMAs that read it have retired (wgmma.wait_group 1)
       int prev_b = -1, prev_a = -1;
       for (int ci = ci0; ci < ci1; ++ci) {
         ptx::mbar_wait(&afull_bar[ia], pha);
-        const uint32_t a0 = ptx::smem_u32(a_ring + ia * Cfg::kAStage) + row_off;
+        const uint32_t a0 = ptx::smem_u32(a_ring + ia * Cfg::kAStage);
         for (int g = 0; g < n_groups; ++g) {
           ptx::mbar_wait(&bfull_bar[ib], phb);
-          if (threadIdx.x == 128 && ci == ci0 && g == 0) trace_tile(p, lt, 1);
+          if (wg_leader && ci == ci0 && g == 0) trace_tile(p, lt, 1);
           ptx::wgmma_fence();
           const int tap0 = g * Cfg::kTPS;
-          const int tap1 = (tap0 + Cfg::kTPS < p.n_taps) ? tap0 + Cfg::kTPS : p.n_taps;
           const uint32_t b0 = ptx::smem_u32(b_ring + ib * Cfg::kBStage);
-          for (int tap = tap0; tap < tap1; ++tap) {
-            const uint32_t a_hi_addr = a0 + static_cast<uint32_t>(p.tap_row[tc.z][tap]) * 128u;
-            const uint32_t b_hi_addr = b0 + static_cast<uint32_t>(tap - tap0) * (NL * Cfg::kBTile);
-            const uint64_t a_hi = ptx::gmma_desc_sw128(a_hi_addr, sbo, boff);
-            const uint64_t b_hi = ptx::gmma_desc_sw128(b_hi_addr);
 #pragma unroll
-            for (int k = 0; k < kChunk / 16; ++k) {
-              const uint32_t accum = (ci > ci0 || tap > 0 || k > 0) ? 1u : 0u;
-              ptx::wgmma_m64k16<BN, NL == 2>(acc, a_hi + 2 * k, b_hi + 2 * k, accum);
-              if constexpr (NL == 2) {
-                const uint64_t a_lo = ptx::gmma_desc_sw128(a_hi_addr + kPatchStride, sbo, boff);
-                const uint64_t b_lo = ptx::gmma_desc_sw128(b_hi_addr + Cfg::kBTile);
-                ptx::wgmma_m64k16<BN, true>(acc, a_hi + 2 * k, b_lo + 2 * k, 1u);
-                ptx::wgmma_m64k16<BN, true>(acc, a_lo + 2 * k, b_hi + 2 * k, 1u);
+          for (int i = 0; i < Cfg::kTPS; ++i) {
+            const int tap = tap0 + i;
+            if (i == 0 || tap < p.n_taps) {                     // the last group may be short (never empty)
+              const uint32_t a_hi_addr = a0 + static_cast<uint32_t>(p.tap_row[tc.z][tap]) * 128u;
+              const uint32_t b_hi_addr = b0 + static_cast<uint32_t>(i) * (NL * Cfg::kBTile);
+              const uint64_t b_hi = ptx::gmma_desc_sw128(b_hi_addr);
+              const uint64_t b_lo = ptx::gmma_desc_sw128(b_hi_addr + Cfg::kBTile);   // PARITY only
+#pragma unroll
+              for (int k = 0; k < kChunk / 16; ++k) {
+                const uint32_t accum = (ci > ci0 || tap > 0 || k > 0) ? 1u : 0u;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                  const uint64_t a_hi = ptx::gmma_desc_sw128(a_hi_addr + h * row_off, sbo, boff);
+                  ptx::wgmma_m64k16<BN, NL == 2>(acc[h], a_hi + 2 * k, b_hi + 2 * k, accum);
+                  if constexpr (NL == 2) {
+                    const uint64_t a_lo = ptx::gmma_desc_sw128(a_hi_addr + h * row_off + kPatchStride, sbo, boff);
+                    ptx::wgmma_m64k16<BN, true>(acc[h], a_hi + 2 * k, b_lo + 2 * k, 1u);
+                    ptx::wgmma_m64k16<BN, true>(acc[h], a_lo + 2 * k, b_hi + 2 * k, 1u);
+                  }
+                }
               }
             }
           }
           ptx::wgmma_commit();
+          if (ci == ci1 - 1 && g == n_groups - 1 && wg_leader) ptx::mbar_arrive(&turn_bar[wg]);   // tile fully issued
           ptx::wgmma_wait<1>();
           if (wg_leader) {
             if (prev_b >= 0) release_stage<CL>(&bempty_bar[prev_b]);
@@ -709,9 +760,11 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
         if (prev_b >= 0) release_stage<CL>(&bempty_bar[prev_b]);
         if (prev_a >= 0) ptx::mbar_arrive(&aempty_bar[prev_a]);
       }
-      if (threadIdx.x == 128) trace_tile(p, lt, 2);
-      epilogue_regs<BN, NL, TAIL>(p, acc, tc, t, cw, tail_stg);
-      if (threadIdx.x == 128) trace_tile(p, lt, 3);
+      if (wg_leader) trace_tile(p, lt, 2);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        epilogue_regs<BN, NL, TAIL>(p, acc[h], tc, t, 64 * h, stg + 64 * h * kTailStride, 1 + wg);
+      if (wg_leader) trace_tile(p, lt, 3);
     }
   }
   if (CL > 1) ptx::cluster_sync();     // no CTA leaves while a peer may still signal its barriers / write its smem
