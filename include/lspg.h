@@ -136,6 +136,7 @@ typedef struct lspg_layer_geo {
   int n_split, split_len, k_items;   /* split-K: K loop of k_items cut into n_split ranges of split_len */
   int ctas;              /* CTAs launched = min(tiles * n_split, SMs) */
   int64_t partial_bytes; /* fp32 split-K partials this layer needs in the scratch region (summed by the finisher kernel) */
+  int cluster;           /* CTAs per thread-block cluster (2: conv_patch_kernel pairs sharing weight tiles by multicast) */
 } lspg_layer_geo;
 int lspg_debug_layer_geo(lspg_handle h, int layer, int batch, int height, int width, lspg_layer_geo* out);
 

@@ -50,7 +50,7 @@ class LspgLayerInfo(C.Structure):
 class LspgLayerGeo(C.Structure):
     _fields_ = [("kernel", C.c_int), ("bn", C.c_int), ("tile_w", C.c_int), ("tile_h", C.c_int), ("tile_n", C.c_int),
                 ("m_tiles", C.c_int), ("n_tiles", C.c_int), ("n_phases", C.c_int), ("n_split", C.c_int), ("split_len", C.c_int),
-                ("k_items", C.c_int), ("ctas", C.c_int), ("partial_bytes", C.c_int64)]
+                ("k_items", C.c_int), ("ctas", C.c_int), ("partial_bytes", C.c_int64), ("cluster", C.c_int)]
 
 
 class LspgError(RuntimeError):

@@ -468,6 +468,7 @@ struct Geo {
   int bn, m_tiles, n_tiles, tiles_per_split;
   int k_items;                 // K-loop length: K blocks (v1) or (source, chunk) items (patch)
   int n_split, split_len;
+  int cluster;                 // CTAs per cluster sharing weight tiles by TMA multicast (patch kernel only)
   size_t partial_bytes;
 };
 
@@ -508,6 +509,9 @@ Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
       else g.split_len = g.k_items;
     }
   }
+  // A 2-CTA cluster pairs neighbouring M tiles, so it needs an even M-tile count, no split-K and a full wave of tiles.
+  static const bool no_cluster = getenv("LSPG_NO_CLUSTER") != nullptr;
+  g.cluster = (g.patch && !no_cluster && g.n_split == 1 && g.m_tiles % 2 == 0 && g.tiles_per_split >= sms) ? 2 : 1;
   return g;
 }
 
@@ -699,8 +703,7 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     const int used = (L.kind == K_S2) ? 4 : L.n_src;
     for (int q = used; q < 4; ++q) p.a[q] = p.a[0];
     if (pl.patch) {
-      static const bool no_cluster = getenv("LSPG_NO_CLUSTER") != nullptr;
-      pl.cluster = ((!no_cluster && g.n_split == 1 && g.m_tiles % 2 == 0 && g.tiles_per_split >= h->num_sms)) ? 2 : 1;
+      pl.cluster = g.cluster;
       if (pl.cluster == 1 && NL == 1) rc = make_weight_map_taps(h, &p.w, L, pl.bn, patch_tps(pl.bn, NL, L.kind == K_TAIL), NL);
       else rc = make_weight_map_taps(h, &p.w, L, pl.bn / pl.cluster, 1, NL);      // per-tap boxes (row slice per CTA when multicasting)
       if (rc) return rc;
@@ -1273,6 +1276,8 @@ int lspg_debug_layer_geo(lspg_handle h, int layer, int batch, int height, int wi
   o->n_split = g.n_split; o->split_len = g.split_len; o->k_items = g.k_items;
   const int sms = h->num_sms_or_default();
   o->ctas = std::min(g.tiles_per_split * g.n_split, sms);
+  o->ctas -= o->ctas % g.cluster;
+  o->cluster = g.cluster;
   o->partial_bytes = static_cast<int64_t>(g.partial_bytes);
   return LSPG_OK;
 }

@@ -237,6 +237,9 @@ def test_planner_invariants(variant, batch):
         else:
             assert g.partial_bytes == 0
         assert 1 <= g.ctas <= sms
+        assert g.cluster in (1, 2)
+        if g.cluster == 2:                                                  # multicast pairs of neighbouring M tiles
+            assert g.kernel == 1 and g.n_split == 1 and g.m_tiles % 2 == 0 and g.ctas % 2 == 0
     assert ws > max(g.partial_bytes for _, g in table)
     n_split_layers = sum(1 for _, g in table if g.n_split > 1)
     assert n_split_layers >= 10 and (batch != 1 or n_split_layers >= 40)
