@@ -134,9 +134,11 @@ typedef struct lspg_layer_geo {
   int tile_w, tile_h, tile_n;   /* output tile = tile_w x tile_h pixels x tile_n images = 128 rows */
   int m_tiles, n_tiles, n_phases;
   int n_split, split_len, k_items;   /* split-K: K loop of k_items cut into n_split ranges of split_len */
-  int ctas;              /* CTAs launched = min(tiles * n_split, SMs) */
+  int ctas;              /* CTAs launched = min(tiles * n_split, SMs), rounded down to whole clusters */
   int64_t partial_bytes; /* fp32 split-K partials this layer needs in the scratch region (summed by the finisher kernel) */
   int cluster;           /* CTAs per thread-block cluster (2: conv_patch_kernel pairs sharing weight tiles by multicast) */
+  int w_box_taps[2];     /* [LSPG_MODE_FAST], [LSPG_MODE_PARITY]: taps per weight TMA box (taps per B stage of conv_patch_kernel
+                            when a FAST stage is one box, else 1) */
 } lspg_layer_geo;
 int lspg_debug_layer_geo(lspg_handle h, int layer, int batch, int height, int width, lspg_layer_geo* out);
 

@@ -15,17 +15,18 @@
 //   * B tiles come from a packed weight tensor [phase*limb][Cout][K] (K-major), same 128B-swizzled layout.
 //   * Warp specialisation: warpgroup 0 = TMA producer (one warp), warpgroups 1 and 2 = consumers issuing
 //     wgmma.m64nBNk16 with fp32 accumulators in registers, then running the epilogue from those registers: folded
-//     eval-BatchNorm scale/shift in fp32, residual, ReLU, 16-bit (hi, lo) NHWC stores.  The tail variant applies tanh
-//     and scatters fp32 NCHW or uint8 HWC directly.
+//     eval-BatchNorm scale/shift in fp32, residual, ReLU, 16-bit (hi, lo) NHWC stores.  The tail variant (patch kernel
+//     only) applies tanh and scatters fp32 NCHW or uint8 HWC directly.
 //     conv_umma_kernel: consumer w owns rows [64w, 64w+64) of every tile.  conv_patch_kernel: ping-pong, consumer w
 //     owns every other tile (all 128 rows, two accumulators), so its epilogue runs under the other one's MMAs.
 //   * NL = 2 ("parity" precision): activations and weights are split into fp16 hi + lo limbs; each K step issues
 //     hi*hi + hi*lo + lo*hi into one accumulator (22 mantissa bits per operand, fp32 accumulate) and the epilogue writes
 //     both limbs.  NL = 1 ("fast"): one bf16 limb, one MMA per K step.
 //
-// Two kernels share the consumer code: conv_umma_kernel (one TMA box per tap; stride-2 convs and everything below 16x16)
-// and conv_patch_kernel (one halo patch per chunk; every other layer, optionally as a 2-CTA cluster that multicasts the
-// weight tiles).  Both are persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...
+// Two conv kernels: conv_umma_kernel (one TMA box per tap; stride-2 convs and grids narrower than 8 or shorter than 16)
+// and conv_patch_kernel (one halo patch per chunk; every other layer including the tail, optionally as a 2-CTA cluster
+// that multicasts the weight tiles).  Both are persistent: each CTA walks tiles blockIdx.x, +gridDim.x, ...  Both, and the
+// split-K finisher splitk_reduce_kernel, apply the regular epilogue through one helper, epilogue_pair.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -97,7 +98,6 @@ struct alignas(64) ConvParams {
   // patch mode: one halo patch {64 ch, patch_w, patch_h} per (tile, source, chunk) whose origin is the tile origin +
   // (patch_dx0, patch_dy0)[phase]; every tap is a row offset inside the patch.
   int32_t patch_w, patch_h;
-  int32_t desc_base_offset;      // 1: set the wgmma descriptor base-offset field from the start address (bring-up switch)
   int8_t patch_dx0[4], patch_dy0[4];
   int16_t tap_row[4][kMaxTaps];  // [phase][tap] -> first patch row of the tap's shifted A tile
   int8_t tap_map[4][kMaxTaps];   // [phase][tap] -> index into a[] (added to the concat source index)
@@ -108,28 +108,26 @@ struct alignas(64) ConvParams {
   CUtensorMap w;             // packed weights, dims {K, Cout_pad, limb*n_phases + phase} (patch kernel: {kc, Cout, tap, limb*phase})
 };
 
-// Shared-memory regions after the operand rings: barriers, then (tail) the accumulator staging of the tail epilogue,
-// kTailRows rows (one tile for the per-tap kernel, whose consumers split every tile; one tile per consumer warpgroup
-// for the patch kernel, whose consumers own whole tiles).
+// Shared-memory regions after the operand rings: barriers, then (patch kernel, tail) the accumulator staging of the tail
+// epilogue, one tile per consumer warpgroup (its consumers own whole tiles).
 constexpr int kBarBytes = 1024;
 constexpr int kTailStride = 17;                                      // floats per staged tail row (16 + 1: no bank conflicts)
-template <bool TAIL, int kTailRows = kTileM>
+template <bool TAIL>
 struct AuxCfg {
-  static constexpr int kTailBytes = TAIL ? kTailRows * kTailStride * 4 : 0;
+  static constexpr int kTailBytes = TAIL ? 2 * kTileM * kTailStride * 4 : 0;
   static constexpr int kBytes = kBarBytes + kTailBytes;
 };
 
-template <int BN, int NL, bool TAIL>
+template <int BN, int NL>
 struct ConvCfg {
-  using Aux = AuxCfg<TAIL>;
   static constexpr int kBTile = BN * 128;
   static constexpr int kStage = NL * (kATile + kBTile);
-  static constexpr int kAvail = kSmemBudget - 1024 /*alignment slack*/ - Aux::kBytes;
+  static constexpr int kAvail = kSmemBudget - 1024 /*alignment slack*/ - kBarBytes;
   static constexpr int kStagesRaw = kAvail / kStage;
   static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kSmemBytes = 1024 + kStages * kStage + Aux::kBytes;
+  static constexpr int kSmemBytes = 1024 + kStages * kStage + kBarBytes;
   static_assert(kStages >= 2, "pipeline needs at least two stages");
-  static_assert(BN == 16 || BN == 64 || BN == 128, "instantiated N tiles");
+  static_assert(BN == 64 || BN == 128, "instantiated N tiles");
 };
 
 // Debug trace layout per CTA: [0] kernel entry, [1] prologue done, [2]/[3] globaltimer (ns) at entry/exit, then per
@@ -221,6 +219,35 @@ __device__ __forceinline__ void row_pixel(const ConvParams& p, const TileCoord& 
   n = tc.n0 + (row >> (p.tw_log2 + p.th_log2));
 }
 
+// Channel 0 of sampling-grid pixel (n, y, x) in the NHWC output (limb 0): with a folded x2 upsample, phase tc.z of it.
+__device__ __forceinline__ __nv_bfloat16* out_pixel(const ConvParams& p, const TileCoord& tc, int n, int y, int x) {
+  const int oh = p.out_up ? 2 * p.hs : p.hs, ow = p.out_up ? 2 * p.ws : p.ws;
+  const int oy = p.out_up ? 2 * y + (tc.z >> 1) : y, ox = p.out_up ? 2 * x + (tc.z & 1) : x;
+  return p.out_ptr + ((static_cast<size_t>(n) * oh + oy) * ow + ox) * p.out_channels;
+}
+
+// Regular epilogue of channel pair j of a pixel, whose channels start at out[kStride * j] (limb 0) and, in PARITY, at
+// out[out_limb_stride + kStride * j]: folded BatchNorm fma, the residual's limbs in limb order (rw[l][j] = the pair's
+// word of limb l, read only if p.has_res), ReLU, then the 16-bit hi word and the lo word of the remainder y - hi.
+template <int kStride, int NL, int M>
+__device__ __forceinline__ void epilogue_pair(const ConvParams& p, float a0, float a1, float2 s2, float2 f2,
+                                              const uint32_t (&rw)[NL][M], int j, __nv_bfloat16* out) {
+  float y0 = fmaf(a0, s2.x, f2.x);
+  float y1 = fmaf(a1, s2.y, f2.y);
+  if (p.has_res) {
+#pragma unroll
+    for (int l = 0; l < NL; ++l) {
+      y0 += unpack_lo<NL == 2>(rw[l][j]);
+      y1 += unpack_hi<NL == 2>(rw[l][j]);
+    }
+  }
+  if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
+  const uint32_t o = pack2<NL == 2>(y0, y1);
+  *reinterpret_cast<uint32_t*>(out + kStride * j) = o;
+  if (NL == 2)
+    *reinterpret_cast<uint32_t*>(out + p.out_limb_stride + kStride * j) = pack2<true>(y0 - unpack_lo<true>(o), y1 - unpack_hi<true>(o));
+}
+
 // Consumer epilogue of the 64 tile rows [rb, rb+64) held by one m64nBN accumulator of the calling warpgroup.
 // Thread layout of the m64nBN accumulator: rows r0 = 16*warp + lane/4 and r0 + 8, columns 8j + 2*(lane%4) and +1
 // (d[4j], d[4j+1] for r0; d[4j+2], d[4j+3] for r0 + 8).
@@ -308,9 +335,7 @@ __device__ __forceinline__ void epilogue_regs(const ConvParams& p, const float (
       int pn, py_, px_;
       row_pixel(p, tc, r0 + 8 * h, pn, py_, px_);
       if (pn >= p.batch || py_ >= p.hs || px_ >= p.ws) continue;
-      const int oh = p.out_up ? 2 * p.hs : p.hs, ow = p.out_up ? 2 * p.ws : p.ws;
-      const int oy = p.out_up ? 2 * py_ + (tc.z >> 1) : py_, ox = p.out_up ? 2 * px_ + (tc.z & 1) : px_;
-      __nv_bfloat16* out_row = p.out_ptr + ((static_cast<size_t>(pn) * oh + oy) * ow + ox) * p.out_channels + tc.nt * BN + c0;
+      __nv_bfloat16* out_row = out_pixel(p, tc, pn, py_, px_) + tc.nt * BN + c0;
       const __nv_bfloat16* res_row =
           p.has_res ? p.res_ptr + ((static_cast<size_t>(pn) * p.hs + py_) * p.ws + px_) * p.res_channels + tc.nt * BN + c0 : nullptr;
       const float* sc = p.scale + tc.nt * BN + c0;
@@ -328,21 +353,7 @@ __device__ __forceinline__ void epilogue_regs(const ConvParams& p, const float (
       for (int j = 0; j < BN / 8; ++j) {
         const float2 s2 = __ldg(reinterpret_cast<const float2*>(sc + 8 * j));
         const float2 f2 = __ldg(reinterpret_cast<const float2*>(sf + 8 * j));
-        float y0 = fmaf(acc[4 * j + 2 * h], s2.x, f2.x);
-        float y1 = fmaf(acc[4 * j + 2 * h + 1], s2.y, f2.y);
-        if (p.has_res) {
-#pragma unroll
-          for (int l = 0; l < NL; ++l) {
-            y0 += unpack_lo<NL == 2>(rw[l][j]);
-            y1 += unpack_hi<NL == 2>(rw[l][j]);
-          }
-        }
-        if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
-        const uint32_t o = pack2<NL == 2>(y0, y1);
-        *reinterpret_cast<uint32_t*>(out_row + 8 * j) = o;
-        if (NL == 2)
-          *reinterpret_cast<uint32_t*>(out_row + p.out_limb_stride + 8 * j) =
-              pack2<true>(y0 - unpack_lo<true>(o), y1 - unpack_hi<true>(o));
+        epilogue_pair<8>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], s2, f2, rw, j, out_row);
       }
     }
   }
@@ -359,16 +370,15 @@ __device__ __forceinline__ void release_stage(uint64_t* bar) {
   }
 }
 
-template <int BN, int NL, bool TAIL>
+template <int BN, int NL>
 __global__ void __launch_bounds__(kThreads, 1) conv_umma_kernel(const __grid_constant__ ConvParams p) {
-  using Cfg = ConvCfg<BN, NL, TAIL>;
+  using Cfg = ConvCfg<BN, NL>;
   const int t0 = static_cast<int>(blockIdx.x), tstep = static_cast<int>(gridDim.x);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* aux = smem + Cfg::kStages * Cfg::kStage;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(aux);   // [kStages]
   uint64_t* empty_bar = full_bar + Cfg::kStages;           // [kStages]
-  float* tail_stg = reinterpret_cast<float*>(aux + kBarBytes);
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // provably warp-uniform
   const int lane = threadIdx.x & 31;
@@ -496,7 +506,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_umma_kernel(const __grid_con
       ptx::wgmma_wait<0>();
       if (prev >= 0 && wg_leader) release_stage<1>(&empty_bar[prev]);
       if (threadIdx.x == 128) trace_tile(p, lt, 2);
-      epilogue_regs<BN, NL, TAIL>(p, acc, tc, t, 64 * cw, tail_stg + cw * 64 * kTailStride, 1 + cw);
+      epilogue_regs<BN, NL, false>(p, acc, tc, t, 64 * cw, nullptr, 0);
       if (threadIdx.x == 128) trace_tile(p, lt, 3);
     }
   }
@@ -528,7 +538,7 @@ static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file
 
 template <int BN, int NL, bool TAIL>
 struct PatchCfg {
-  using Aux = AuxCfg<TAIL, 2 * kTileM>;
+  using Aux = AuxCfg<TAIL>;
   static constexpr int kBTile = BN * 128;
   // taps per B stage: each stage costs one barrier round trip, so a stage must carry enough tensor work: 2 taps for
   // N=128 bf16, 2-3 for N=64, all 9 for the tail.
@@ -683,7 +693,6 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
     uint32_t pha = 0, phb = 0;
     const uint32_t sbo = static_cast<uint32_t>(p.patch_w) * 128u;
     const uint32_t row_off = static_cast<uint32_t>(8 * p.patch_w) * 128u;   // tile rows 64..127: 8 image rows down
-    const bool boff = p.desc_base_offset != 0;
     float* stg = tail_stg + wg * kTileM * kTailStride;                       // this warpgroup's tail staging (128 rows)
     int lt = 0;
     for (int t = t0; t < p.total_tiles; t += tstep, ++lt) {
@@ -731,10 +740,10 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
                 const uint32_t accum = (ci > ci0 || tap > 0 || k > 0) ? 1u : 0u;
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
-                  const uint64_t a_hi = ptx::gmma_desc_sw128(a_hi_addr + h * row_off, sbo, boff);
+                  const uint64_t a_hi = ptx::gmma_desc_sw128(a_hi_addr + h * row_off, sbo);
                   ptx::wgmma_m64k16<BN, NL == 2>(acc[h], a_hi + 2 * k, b_hi + 2 * k, accum);
                   if constexpr (NL == 2) {
-                    const uint64_t a_lo = ptx::gmma_desc_sw128(a_hi_addr + h * row_off + kPatchStride, sbo, boff);
+                    const uint64_t a_lo = ptx::gmma_desc_sw128(a_hi_addr + h * row_off + kPatchStride, sbo);
                     ptx::wgmma_m64k16<BN, true>(acc[h], a_hi + 2 * k, b_lo + 2 * k, 1u);
                     ptx::wgmma_m64k16<BN, true>(acc[h], a_lo + 2 * k, b_hi + 2 * k, 1u);
                   }
@@ -775,26 +784,16 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
 // Split-K finisher: out = epilogue( sum_s partial[s] ).
 // Memory-bound and tiny (the layers that use split-K have at most a few hundred output pixels per image).
 // ====================================================================================================
-struct ReduceParams {
-  const float* partial;
-  const float* scale;
-  const float* shift;
-  const __nv_bfloat16* res;
-  long long res_limb_stride;      // elements
-  __nv_bfloat16* out;
-  long long out_limb_stride;
-  int32_t n_split, tiles_per_split, m_tiles, n_tiles, n_phases;
-  int32_t tiles_x, tiles_y, tw_log2, th_log2, bn;
-  int32_t batch, hs, ws, up, channels, relu, has_res, nl;
-};
-
 // One thread = one pixel x 4 channels.  The layers that use split-K are latency bound (a few hundred output pixels, 8-36
 // splits): what matters is how many dependent trips to L2 the sum takes, so up to 16 splits are in flight per trip
 // (round 1 summed 4 per trip over 8-channel groups: 6 dependent trips for 18 splits, as long as the conv itself at batch 1).
-__global__ void __launch_bounds__(128) splitk_reduce_kernel(const ReduceParams p) {
+// It reads the conv launch's own parameters; the split-K layers are never the tail, so the output has Cout_pad channels.
+template <int NL>
+__global__ void __launch_bounds__(128) splitk_reduce_kernel(const __grid_constant__ ConvParams p) {
   ptx::pdl_wait();
   ptx::pdl_launch_dependents();
-  const int groups = p.bn >> 2;
+  const int bn = p.out_channels / p.n_tiles;
+  const int groups = bn >> 2;
   const long long total = static_cast<long long>(p.tiles_per_split) * kTileM * groups;
   for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < total;
        e += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -802,23 +801,13 @@ __global__ void __launch_bounds__(128) splitk_reduce_kernel(const ReduceParams p
     const long long r0 = e / groups;
     const int row = static_cast<int>(r0 % kTileM);
     const int tile = static_cast<int>(r0 / kTileM);
-    const int mt = tile % p.m_tiles;
-    const int r1 = tile / p.m_tiles;
-    const int nt = r1 % p.n_tiles;
-    const int z = r1 / p.n_tiles;
-    const int tx = mt % p.tiles_x;
-    const int r2 = mt / p.tiles_x;
-    const int ty = r2 % p.tiles_y;
-    const int tn = r2 / p.tiles_y;
-    const int tw = row & ((1 << p.tw_log2) - 1);
-    const int th = (row >> p.tw_log2) & ((1 << p.th_log2) - 1);
-    const int nb = row >> (p.tw_log2 + p.th_log2);
-    const int n = (tn << (7 - p.tw_log2 - p.th_log2)) + nb;
-    const int y = (ty << p.th_log2) + th, x = (tx << p.tw_log2) + tw;
+    const TileCoord tc = decode_tile(p, tile);       // split 0: tile < tiles_per_split
+    int n, y, x;
+    row_pixel(p, tc, row, n, y, x);
     if (n >= p.batch || y >= p.hs || x >= p.ws) continue;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
-    const size_t split_stride = static_cast<size_t>(p.tiles_per_split) * kTileM * p.bn;      // floats between splits
-    const float* src0 = p.partial + (static_cast<size_t>(tile) * kTileM + row) * p.bn + g * 4;
+    const size_t split_stride = static_cast<size_t>(p.tiles_per_split) * kTileM * bn;      // floats between splits
+    const float* src0 = p.partial + (static_cast<size_t>(tile) * kTileM + row) * bn + g * 4;
     int s = 0;
     for (; s + 16 <= p.n_split; s += 16) {     // sixteen independent 16-byte loads in flight
       float4 v[16];
@@ -840,38 +829,20 @@ __global__ void __launch_bounds__(128) splitk_reduce_kernel(const ReduceParams p
       const float4 a = *reinterpret_cast<const float4*>(src0 + s * split_stride);
       acc[0] += a.x; acc[1] += a.y; acc[2] += a.z; acc[3] += a.w;
     }
-    const int ch = nt * p.bn + g * 4;
-    const int oh = p.up ? 2 * p.hs : p.hs, ow = p.up ? 2 * p.ws : p.ws;
-    const int oy = p.up ? 2 * y + (z >> 1) : y, ox = p.up ? 2 * x + (z & 1) : x;
-    const size_t off = ((static_cast<size_t>(n) * oh + oy) * ow + ox) * p.channels + ch;
+    const int ch = tc.nt * bn + g * 4;
+    __nv_bfloat16* out = out_pixel(p, tc, n, y, x) + ch;
     const float4 sc = *reinterpret_cast<const float4*>(p.scale + ch), sh = *reinterpret_cast<const float4*>(p.shift + ch);
-    float yv[4] = {fmaf(acc[0], sc.x, sh.x), fmaf(acc[1], sc.y, sh.y), fmaf(acc[2], sc.z, sh.z), fmaf(acc[3], sc.w, sh.w)};
+    uint32_t rw[NL][2];                          // per limb: residual words of channels (ch, ch+1) and (ch+2, ch+3)
     if (p.has_res) {
-      for (int l = 0; l < p.nl; ++l) {
-        const uint2 r = *reinterpret_cast<const uint2*>(p.res + l * p.res_limb_stride + off);
-        if (p.nl == 2) {                          // PARITY: fp16 limbs
-          yv[0] += unpack_lo<true>(r.x); yv[1] += unpack_hi<true>(r.x); yv[2] += unpack_lo<true>(r.y); yv[3] += unpack_hi<true>(r.y);
-        } else {                                  // FAST: bf16
-          yv[0] += bf16_lo(r.x); yv[1] += bf16_hi(r.x); yv[2] += bf16_lo(r.y); yv[3] += bf16_hi(r.y);
-        }
+      const size_t roff = ((static_cast<size_t>(n) * p.hs + y) * p.ws + x) * p.res_channels + ch;
+#pragma unroll
+      for (int l = 0; l < NL; ++l) {
+        const uint2 r = *reinterpret_cast<const uint2*>(p.res_ptr + l * p.res_limb_stride + roff);
+        rw[l][0] = r.x; rw[l][1] = r.y;
       }
     }
-    if (p.relu) {
-#pragma unroll
-      for (int i = 0; i < 4; ++i) yv[i] = fmaxf(yv[i], 0.f);
-    }
-    if (p.nl == 2) {
-      uint2 o, lo;
-      o.x = pack2<true>(yv[0], yv[1]); o.y = pack2<true>(yv[2], yv[3]);
-      lo.x = pack2<true>(yv[0] - unpack_lo<true>(o.x), yv[1] - unpack_hi<true>(o.x));
-      lo.y = pack2<true>(yv[2] - unpack_lo<true>(o.y), yv[3] - unpack_hi<true>(o.y));
-      *reinterpret_cast<uint2*>(p.out + off) = o;
-      *reinterpret_cast<uint2*>(p.out + p.out_limb_stride + off) = lo;
-    } else {
-      uint2 o;
-      o.x = pack_bf16x2(yv[0], yv[1]); o.y = pack_bf16x2(yv[2], yv[3]);
-      *reinterpret_cast<uint2*>(p.out + off) = o;
-    }
+    epilogue_pair<2>(p, acc[0], acc[1], make_float2(sc.x, sc.y), make_float2(sh.x, sh.y), rw, 0, out);
+    epilogue_pair<2>(p, acc[2], acc[3], make_float2(sc.z, sc.w), make_float2(sh.z, sh.w), rw, 1, out);
   }
 }
 

@@ -17,6 +17,7 @@
 #include <memory>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <utility>
 #include <vector>
 
@@ -103,15 +104,24 @@ struct Layer {
   float* d_shift = nullptr;
 };
 
+// Tiling / kernel-variant decisions of one layer for a problem size (layer_geo; shared by planning, workspace sizing and
+// lspg_debug_layer_geo).
+struct Geo {
+  int hs, ws;                  // sampling grid
+  int tw, th, nb;              // output tile = tw x th pixels x nb images (= 128 rows)
+  bool patch;                  // conv_patch_kernel (halo patch) vs conv_umma_kernel (one box per tap)
+  int bn, m_tiles, n_tiles, tiles_per_split;
+  int k_items;                 // K-loop length: K blocks (v1) or (source, chunk) items (patch)
+  int n_split, split_len;      // split-K (n_split > 1): the conv writes fp32 partials, splitk_reduce_kernel finishes
+  int cluster;                 // CTAs per cluster sharing weight tiles by TMA multicast (patch kernel only)
+  int ctas;                    // launch grid: one persistent CTA per tile up to one per SM, whole clusters
+  size_t partial_bytes;
+};
+
 struct PlanLayer {
   ConvParams prm;
-  int bn = 64;
-  int grid = 1;
-  bool patch = false;     // conv_patch_kernel (halo patch per chunk) instead of conv_umma_kernel (one box per tap)
-  int cluster = 1;        // CTAs per cluster sharing B stages by TMA multicast (patch mode only)
-  bool split = false;     // split-K: conv kernel writes fp32 partials, splitk_reduce_kernel finishes
-  ReduceParams red;
-  int red_blocks = 0;
+  Geo g;
+  int red_blocks = 0;     // split-K finisher grid
 };
 
 struct IoKey {
@@ -460,21 +470,7 @@ int ilog2(int v) {
   return l;
 }
 
-// Tiling / kernel-variant decisions of one layer for a problem size (shared by planning and workspace sizing).
-struct Geo {
-  int hs, ws;                  // sampling grid
-  int tw, th, nb;              // output tile = tw x th pixels x nb images (= 128 rows)
-  bool patch;                  // conv_patch_kernel (halo patch) vs conv_umma_kernel (one box per tap)
-  int bn, m_tiles, n_tiles, tiles_per_split;
-  int k_items;                 // K-loop length: K blocks (v1) or (source, chunk) items (patch)
-  int n_split, split_len;
-  int cluster;                 // CTAs per cluster sharing weight tiles by TMA multicast (patch kernel only)
-  size_t partial_bytes;
-};
-
 Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
-  static const bool no_patch = getenv("LSPG_NO_PATCH") != nullptr;
-  static const bool no_split = getenv("LSPG_NO_SPLITK") != nullptr;
   Geo g;
   g.hs = H >> L.grid_shift; g.ws = W >> L.grid_shift;
   g.tw = g.ws < 16 ? g.ws : 16;
@@ -482,7 +478,7 @@ Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
   if (g.th > g.hs) g.th = g.hs;
   g.nb = 128 / (g.tw * g.th);
   // patch mode needs 8-pixel-wide tiles (one 8-row core-matrix group of the wgmma A operand = one image row of the halo patch)
-  g.patch = !no_patch && L.kind != K_S2 && g.ws >= 8 && g.hs >= 16;
+  g.patch = L.kind != K_S2 && g.ws >= 8 && g.hs >= 16;
   if (g.patch) { g.tw = 8; g.th = 16; g.nb = 1; }
   g.m_tiles = (g.ws / g.tw) * (g.hs / g.th) * ((B + g.nb - 1) / g.nb);
   const int chunks = L.cin[0] / 64 + (L.n_src == 2 ? L.cin[1] / 64 : 0);
@@ -496,7 +492,7 @@ Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
   g.tiles_per_split = g.m_tiles * g.n_tiles * L.n_phases;
   g.n_split = 1; g.split_len = g.k_items; g.partial_bytes = 0;
   const int sms = h->num_sms_or_default();
-  if (!no_split && L.kind != K_TAIL && g.tiles_per_split * 2 <= sms) {
+  if (L.kind != K_TAIL && g.tiles_per_split * 2 <= sms) {
     const int min_len = g.patch ? 1 : 4;                       // at least 4 K blocks (v1) / 1 chunk of all taps per split
     int want = sms / g.tiles_per_split;                        // floor: tiles x splits stay within one wave
     int max_split = g.k_items / min_len;
@@ -510,8 +506,9 @@ Geo layer_geo(const lspg_ctx* h, const Layer& L, int B, int H, int W) {
     }
   }
   // A 2-CTA cluster pairs neighbouring M tiles, so it needs an even M-tile count, no split-K and a full wave of tiles.
-  static const bool no_cluster = getenv("LSPG_NO_CLUSTER") != nullptr;
-  g.cluster = (g.patch && !no_cluster && g.n_split == 1 && g.m_tiles % 2 == 0 && g.tiles_per_split >= sms) ? 2 : 1;
+  g.cluster = (g.patch && g.n_split == 1 && g.m_tiles % 2 == 0 && g.tiles_per_split >= sms) ? 2 : 1;
+  g.ctas = std::min(g.tiles_per_split * g.n_split, sms);
+  g.ctas -= g.ctas % g.cluster;
   return g;
 }
 
@@ -609,10 +606,52 @@ int make_weight_map_taps(lspg_ctx* h, CUtensorMap* m, const Layer& L, int bn, in
   return LSPG_OK;
 }
 
-int patch_tps(int bn, int NL, bool tail) {   // must mirror PatchCfg::kTPS
-  if (tail) return 9;
-  if (bn >= 128) return NL == 1 ? 2 : 1;
-  return NL == 1 ? 3 : 2;
+// The kernel instantiation of one layer variant: conv_patch_kernel (PATCH) or conv_umma_kernel, N tile, limbs, tail
+// epilogue, CTAs per cluster.
+template <bool PATCH, int BN, int NL, bool TAIL, int CL>
+struct ConvKernel {
+  static constexpr int kCluster = CL;
+  static constexpr auto kernel() {
+    if constexpr (PATCH) return conv_patch_kernel<BN, NL, TAIL, CL>;
+    else return conv_umma_kernel<BN, NL>;
+  }
+  static constexpr int smem_bytes() {
+    if constexpr (PATCH) return PatchCfg<BN, NL, TAIL>::kSmemBytes;
+    else return ConvCfg<BN, NL>::kSmemBytes;
+  }
+  // Taps per weight TMA box: without multicast the patch kernel fetches a FAST B stage (kTPS taps) as one box; every other
+  // launch fetches one tap per box.
+  static constexpr int box_taps() {
+    if constexpr (PATCH && CL == 1 && NL == 1) return PatchCfg<BN, NL, TAIL>::kTPS;
+    else return 1;
+  }
+};
+
+// Calls f(ConvKernel<...>{}) for a layer variant: the one map from a planned (patch, bn, NL, tail, cluster) to a kernel
+// instantiation.  The per-tap kernel has no tail or cluster variant: layer_geo gives the tail to the patch kernel and
+// clusters only to patch layers.
+template <typename F>
+auto with_conv_kernel(bool patch, int bn, int NL, bool tail, int cluster, F&& f) {
+  const auto nl_cl = [&](auto patch_c, auto bn_c, auto tail_c) {
+    constexpr bool P = decltype(patch_c)::value, T = decltype(tail_c)::value;
+    constexpr int BN = decltype(bn_c)::value;
+    if constexpr (P) {
+      if (cluster == 2) return NL == 1 ? f(ConvKernel<P, BN, 1, T, 2>{}) : f(ConvKernel<P, BN, 2, T, 2>{});
+    }
+    return NL == 1 ? f(ConvKernel<P, BN, 1, T, 1>{}) : f(ConvKernel<P, BN, 2, T, 1>{});
+  };
+  using Yes = std::true_type;
+  using No = std::false_type;
+  using N16 = std::integral_constant<int, 16>;
+  using N64 = std::integral_constant<int, 64>;
+  using N128 = std::integral_constant<int, 128>;
+  if (!patch) return bn == 128 ? nl_cl(No{}, N128{}, No{}) : nl_cl(No{}, N64{}, No{});
+  if (tail) return nl_cl(Yes{}, N16{}, Yes{});
+  return bn == 128 ? nl_cl(Yes{}, N128{}, No{}) : nl_cl(Yes{}, N64{}, No{});
+}
+
+int w_box_taps(const Geo& g, bool tail, int NL) {
+  return with_conv_kernel(g.patch, g.bn, NL, tail, g.cluster, [](auto k) { return decltype(k)::box_taps(); });
 }
 
 int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* workspace) {
@@ -634,13 +673,14 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     ConvParams& p = pl.prm;
     memset(&p, 0, sizeof(p));
     const Geo g = layer_geo(h, L, B, H, W);
+    if (L.kind == K_TAIL && !g.patch) return fail(LSPG_EINVAL, "the tail layer needs the patch kernel (grid %dx%d)", g.hs, g.ws);
+    pl.g = g;
     const int Hs = g.hs, Ws = g.ws;
     const int tw = g.tw, th = g.th, nb = g.nb;
     // The tensor core's swizzle phase follows the absolute smem address (as TMA's does), so a 128-byte-shifted start
     // needs no descriptor base offset.
-    pl.patch = g.patch;
     int abox_w = tw, abox_h = th, abox_n = nb;
-    if (pl.patch) {
+    if (g.patch) {
       int pw = 0, ph = 0;
       for (int z = 0; z < L.n_phases; ++z) {
         int dx0 = 127, dx1 = -127, dy0 = 127, dy1 = -127;
@@ -655,14 +695,12 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
       for (int z = 0; z < L.n_phases; ++z)
         for (int t = 0; t < L.n_taps; ++t)
           p.tap_row[z][t] = static_cast<int16_t>((L.tap_dy[z][t] - p.patch_dy0[z]) * pw + (L.tap_dx[z][t] - p.patch_dx0[z]));
-      p.desc_base_offset = 0;
       if (pw * ph * 128 > kPatchSlot) return fail(LSPG_EINVAL, "patch %dx%d does not fit its smem slot", pw, ph);
       abox_w = pw; abox_h = ph; abox_n = 1;
     }
-    pl.bn = g.bn;
     p.tw_log2 = ilog2(tw); p.th_log2 = ilog2(th);
     p.tiles_x = Ws / tw; p.tiles_y = Hs / th; p.tiles_n = (B + nb - 1) / nb;
-    p.n_tiles = L.cout_pad / pl.bn;
+    p.n_tiles = g.n_tiles;
     p.n_phases = L.n_phases;
     p.tiles_per_split = g.tiles_per_split;
     p.fd_tps = make_fast_div(g.tiles_per_split);
@@ -673,9 +711,8 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     p.n_split = g.n_split; p.split_len = g.split_len;
     p.total_tiles = g.tiles_per_split * g.n_split;
     p.partial = reinterpret_cast<float*>(ws_scratch);
-    // Split-K without a cluster is two-pass: raw fp32 partials, then splitk_reduce_kernel (a grid of threads sums a tile
-    // far faster than the epilogue threads of the last-arriving CTA could).
-    pl.split = g.n_split > 1;
+    // Split-K is two-pass: raw fp32 partials, then splitk_reduce_kernel (a grid of threads sums a tile far faster than the
+    // epilogue threads of the last-arriving CTA could).
     p.n_taps = L.n_taps; p.n_src = L.n_src;
     p.chunks[0] = L.cin[0] / 64; p.chunks[1] = L.n_src == 2 ? L.cin[1] / 64 : 0;
     p.relu = L.relu; p.has_res = L.res >= 0 ? 1 : 0;
@@ -702,13 +739,11 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
     // unused slots still need valid descriptors for prefetch.tensormap
     const int used = (L.kind == K_S2) ? 4 : L.n_src;
     for (int q = used; q < 4; ++q) p.a[q] = p.a[0];
-    if (pl.patch) {
-      pl.cluster = g.cluster;
-      if (pl.cluster == 1 && NL == 1) rc = make_weight_map_taps(h, &p.w, L, pl.bn, patch_tps(pl.bn, NL, L.kind == K_TAIL), NL);
-      else rc = make_weight_map_taps(h, &p.w, L, pl.bn / pl.cluster, 1, NL);      // per-tap boxes (row slice per CTA when multicasting)
-      if (rc) return rc;
+    if (g.patch) {
+      // a row slice of BN/cluster rows per CTA when multicasting
+      if ((rc = make_weight_map_taps(h, &p.w, L, g.bn / g.cluster, w_box_taps(g, L.kind == K_TAIL, NL), NL))) return rc;
     } else {
-      if ((rc = make_weight_map(h, &p.w, L, pl.bn, NL))) return rc;
+      if ((rc = make_weight_map(h, &p.w, L, g.bn, NL))) return rc;
     }
     // ---- output / residual pointers (the epilogue stores and loads them directly)
     if (L.kind != K_TAIL) {
@@ -726,8 +761,6 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
         p.res_channels = r.channels;
       }
     }
-    pl.grid = p.total_tiles < h->num_sms ? p.total_tiles : h->num_sms;
-    if (pl.cluster > 1) pl.grid -= pl.grid % pl.cluster;
     {
       const char* tl = getenv("LSPG_TRACE_LAYER");
       if (tl && atoi(tl) == static_cast<int>(P->layers.size())) {
@@ -738,20 +771,7 @@ int build_plan(lspg_ctx* h, Plan* P, int B, int H, int W, int mode, void* worksp
         p.trace_skip = ts ? atoi(ts) : 0;
       }
     }
-    if (pl.split) {
-      ReduceParams& r = pl.red;
-      memset(&r, 0, sizeof(r));
-      r.partial = p.partial; r.scale = p.scale; r.shift = L.d_shift;
-      r.out = reinterpret_cast<__nv_bfloat16*>(ws + P->tensor_off[L.out]);
-      r.out_limb_stride = static_cast<long long>(P->tensor_limb_stride[L.out] / 2);
-      if (L.res >= 0) {
-        r.res = reinterpret_cast<const __nv_bfloat16*>(ws + P->tensor_off[L.res]);
-        r.res_limb_stride = static_cast<long long>(P->tensor_limb_stride[L.res] / 2);
-      }
-      r.n_split = g.n_split; r.tiles_per_split = g.tiles_per_split; r.m_tiles = g.m_tiles; r.n_tiles = g.n_tiles;
-      r.n_phases = L.n_phases; r.tiles_x = p.tiles_x; r.tiles_y = p.tiles_y; r.tw_log2 = p.tw_log2; r.th_log2 = p.th_log2;
-      r.bn = g.bn; r.batch = B; r.hs = Hs; r.ws = Ws; r.up = (L.kind == K_UP) ? 1 : 0; r.channels = L.cout_pad;
-      r.relu = L.relu; r.has_res = L.res >= 0 ? 1 : 0; r.nl = NL;
+    if (g.n_split > 1) {
       const long long work = static_cast<long long>(g.tiles_per_split) * kTileM * (g.bn / 4);   // one thread per pixel x 4 channels
       pl.red_blocks = static_cast<int>(std::min<long long>((work + 127) / 128, 8LL * h->num_sms));
     }
@@ -806,43 +826,17 @@ int ensure_smem(K kernel, int bytes, int device, unsigned long long* done_mask) 
 
 const void* g_last_func = nullptr;     // host stub of the most recent conv launch (identifies graph nodes after capture)
 
-template <int BN, int NL, bool TAIL>
-int launch_conv(const ConvParams& p, int grid, int device, cudaStream_t st) {
-  using Cfg = ConvCfg<BN, NL, TAIL>;
-  static unsigned long long done = 0;
-  int rc = ensure_smem(conv_umma_kernel<BN, NL, TAIL>, Cfg::kSmemBytes, device, &done);
-  if (rc) return rc;
-  g_last_func = reinterpret_cast<const void*>(conv_umma_kernel<BN, NL, TAIL>);
-  CUDA_TRY(launch_pdl_cluster(conv_umma_kernel<BN, NL, TAIL>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, 1, p));
-  return LSPG_OK;
-}
-
-template <int BN, int NL, bool TAIL, int CL>
-int launch_patch(const ConvParams& p, int grid, int device, cudaStream_t st) {
-  using Cfg = PatchCfg<BN, NL, TAIL>;
-  static unsigned long long done = 0;
-  int rc = ensure_smem(conv_patch_kernel<BN, NL, TAIL, CL>, Cfg::kSmemBytes, device, &done);
-  if (rc) return rc;
-  g_last_func = reinterpret_cast<const void*>(conv_patch_kernel<BN, NL, TAIL, CL>);
-  CUDA_TRY(launch_pdl_cluster(conv_patch_kernel<BN, NL, TAIL, CL>, dim3(grid), dim3(kThreads), Cfg::kSmemBytes, st, CL, p));
-  return LSPG_OK;
-}
-
-template <int BN, int NL, bool TAIL>
-int launch_patch_cl(const ConvParams& p, int grid, int cluster, int device, cudaStream_t st) {
-  return cluster == 2 ? launch_patch<BN, NL, TAIL, 2>(p, grid, device, st) : launch_patch<BN, NL, TAIL, 1>(p, grid, device, st);
-}
-
 int launch_layer(const PlanLayer& pl, int kind, int NL, int device, cudaStream_t st) {
-  if (pl.patch) {
-    const int c = pl.cluster;
-    if (kind == K_TAIL) return NL == 1 ? launch_patch_cl<16, 1, true>(pl.prm, pl.grid, c, device, st) : launch_patch_cl<16, 2, true>(pl.prm, pl.grid, c, device, st);
-    if (pl.bn == 128) return NL == 1 ? launch_patch_cl<128, 1, false>(pl.prm, pl.grid, c, device, st) : launch_patch_cl<128, 2, false>(pl.prm, pl.grid, c, device, st);
-    return NL == 1 ? launch_patch_cl<64, 1, false>(pl.prm, pl.grid, c, device, st) : launch_patch_cl<64, 2, false>(pl.prm, pl.grid, c, device, st);
-  }
-  if (kind == K_TAIL) return NL == 1 ? launch_conv<16, 1, true>(pl.prm, pl.grid, device, st) : launch_conv<16, 2, true>(pl.prm, pl.grid, device, st);
-  if (pl.bn == 128) return NL == 1 ? launch_conv<128, 1, false>(pl.prm, pl.grid, device, st) : launch_conv<128, 2, false>(pl.prm, pl.grid, device, st);
-  return NL == 1 ? launch_conv<64, 1, false>(pl.prm, pl.grid, device, st) : launch_conv<64, 2, false>(pl.prm, pl.grid, device, st);
+  const Geo& g = pl.g;
+  return with_conv_kernel(g.patch, g.bn, NL, kind == K_TAIL, g.cluster, [&](auto k) -> int {
+    using K = decltype(k);
+    static unsigned long long done = 0;       // one per instantiation of this lambda, i.e. per kernel
+    int rc = ensure_smem(K::kernel(), K::smem_bytes(), device, &done);
+    if (rc) return rc;
+    g_last_func = reinterpret_cast<const void*>(K::kernel());
+    CUDA_TRY(launch_pdl_cluster(K::kernel(), dim3(g.ctas), dim3(kThreads), K::smem_bytes(), st, K::kCluster, pl.prm));
+    return LSPG_OK;
+  });
 }
 
 // The caller-dependent arguments of the two I/O nodes of a forward (input packer, tail conv).
@@ -899,15 +893,16 @@ int enqueue_forward(lspg_ctx* h, Plan* P, const IoKey& io, cudaStream_t st, bool
     if (h->layers[i].kind == K_TAIL) set_tail_io(&pl.prm, io);
     if ((rc = launch_layer(pl, h->layers[i].kind, NL, h->device, st))) return rc;
     if (h->layers[i].kind == K_TAIL) h->tail_func = g_last_func;
-    if (pl.split) {
-      CUDA_TRY(launch_pdl(splitk_reduce_kernel, dim3(pl.red_blocks), dim3(128), 0, st, pl.red));
+    if (pl.g.n_split > 1) {
+      if (NL == 1) CUDA_TRY(launch_pdl(splitk_reduce_kernel<1>, dim3(pl.red_blocks), dim3(128), 0, st, pl.prm));
+      else CUDA_TRY(launch_pdl(splitk_reduce_kernel<2>, dim3(pl.red_blocks), dim3(128), 0, st, pl.prm));
     }
     if (evs) CUDA_TRY(cudaEventRecord((*evs)[i + 2], st));
     if (debug_sync) {
       cudaError_t e = cudaStreamSynchronize(st);
       if (e != cudaSuccess)
         return fail(LSPG_ECUDA, "layer %zu (kind %d, %s, bn %d, grid %d, tiles %d) failed: %s", i, h->layers[i].kind,
-                    h->layers[i].conv_key.c_str(), pl.bn, pl.grid, pl.prm.total_tiles, cudaGetErrorString(e));
+                    h->layers[i].conv_key.c_str(), pl.g.bn, pl.g.ctas, pl.prm.total_tiles, cudaGetErrorString(e));
     }
   }
   return LSPG_OK;
@@ -1274,11 +1269,11 @@ int lspg_debug_layer_geo(lspg_handle h, int layer, int batch, int height, int wi
   o->tile_w = g.tw; o->tile_h = g.th; o->tile_n = g.nb;
   o->m_tiles = g.m_tiles; o->n_tiles = g.n_tiles; o->n_phases = L.n_phases;
   o->n_split = g.n_split; o->split_len = g.split_len; o->k_items = g.k_items;
-  const int sms = h->num_sms_or_default();
-  o->ctas = std::min(g.tiles_per_split * g.n_split, sms);
-  o->ctas -= o->ctas % g.cluster;
+  o->ctas = g.ctas;
   o->cluster = g.cluster;
   o->partial_bytes = static_cast<int64_t>(g.partial_bytes);
+  o->w_box_taps[LSPG_MODE_FAST] = w_box_taps(g, L.kind == K_TAIL, nl_of(LSPG_MODE_FAST));
+  o->w_box_taps[LSPG_MODE_PARITY] = w_box_taps(g, L.kind == K_TAIL, nl_of(LSPG_MODE_PARITY));
   return LSPG_OK;
 }
 
@@ -1328,7 +1323,7 @@ int lspg_launches_per_forward(lspg_handle h, int* out) {
   if (!h || !out) return fail(LSPG_EINVAL, "null argument");
   int n = 1 + static_cast<int>(h->layers.size());
   if (h->last_plan)
-    for (const auto& pl : h->last_plan->layers) n += pl.split ? 1 : 0;   // + split-K finishers of the last plan
+    for (const auto& pl : h->last_plan->layers) n += pl.g.n_split > 1 ? 1 : 0;   // + split-K finishers of the last plan
   *out = n;
   return LSPG_OK;
 }

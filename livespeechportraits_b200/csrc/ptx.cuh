@@ -190,14 +190,12 @@ __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sy
 // swizzle (what a TMA box with a 128-byte inner extent and CU_TENSOR_MAP_SWIZZLE_128B writes): `sbo` bytes between 8-row
 // groups (1024 for a dense tile), LBO unused for swizzled K-major layouts, layout type 1 = SWIZZLE_128B in bits [62,64).
 // Advancing K by 16 elements = +32 bytes on the start address (+2 in descriptor units); the hardware applies the XOR
-// swizzle on the final address bits.  `base_off` sets the matrix base-offset field from the start address (bring-up
-// switch; off by default).
-__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes = 1024, bool base_off = false) {
+// swizzle on the final address bits, so the matrix base-offset field stays 0 at any 128-byte-aligned start.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t smem_addr, uint32_t sbo_bytes = 1024) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4);   // start address, 16-byte units, 14 bits
   d |= static_cast<uint64_t>(1) << 16;                        // leading byte offset (ignored; canonical 1)
   d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;           // stride byte offset between 8-row groups
-  if (base_off) d |= static_cast<uint64_t>((smem_addr >> 7) & 7u) << 49;
   d |= static_cast<uint64_t>(1) << 62;                        // SWIZZLE_128B
   return d;
 }

@@ -1,6 +1,6 @@
 #!/bin/bash
 # A/B a bring-up switch with alternating runs on the SAME box (box-to-box variation is +-3 %, larger than most effects).
-# Usage:  bash tests/gpu_scripts/ab.sh "LSPG_NO_CLUSTER=1" [batch] [mode] [rounds]
+# Usage:  bash tests/gpu_scripts/ab.sh "LSPG_NO_PDL=1" [batch] [mode] [rounds]
 # Prints the ms/forward of every run and the medians.
 mkdir -p gpurun_out
 VAR="$1"; B=${2:-32}; MODE=${3:-parity}; N=${4:-3}

@@ -230,6 +230,8 @@ def test_planner_invariants(variant, batch):
         assert g.kernel in (0, 1)
         if g.kernel == 1:
             assert info.kind != 2 and (g.tile_w, g.tile_h) == (8, 16)      # stride-2 convs use the per-tap kernel
+        if info.kind == 4:
+            assert g.kernel == 1                                            # the tail is always the patch kernel
         if g.n_split > 1:
             assert tiles * g.n_split <= sms                                  # split-K never spills into a second wave
             assert (g.n_split - 1) * g.split_len < g.k_items <= g.n_split * g.split_len   # every split has work

@@ -163,11 +163,9 @@ EVERY_LAYER = ("drop_hi_lo", "drop_lo_hi")          # must fail the kernel-arith
 
 def fast_short_tap(info, g):
     """Kernel tap index of the last tap of a short tap group, or None.  In FAST, conv_patch_kernel without a cluster fetches
-    the weights of several taps with one TMA box (taps per stage: csrc/lspg.cu patch_tps), and a last group with fewer
+    the weights of several taps with one TMA box (the planner reports its taps in w_box_taps), and a last group with fewer
     taps than the box is completed by TMA's zero fill."""
-    if g.kernel != 1 or g.cluster != 1:
-        return None
-    tps = 9 if info.kind == R.KIND_TAIL else (2 if g.bn >= 128 else 3)
+    tps = g.w_box_taps[_lib.LSPG_MODE["fast"]]
     return info.n_taps - 1 if info.n_taps % tps else None
 
 
