@@ -204,79 +204,61 @@ BlockKeys block_keys(const std::string& prefix, bool outer, bool inner, int nres
   return b;
 }
 
-void set_taps_s1(Layer& L) {
-  L.n_phases = 1;
-  L.n_taps = 9;
-  for (int r = 0; r < 3; ++r)
-    for (int s = 0; s < 3; ++s) {
-      L.tap_map[0][r * 3 + s] = 0;
-      L.tap_dx[0][r * 3 + s] = static_cast<int8_t>(s - 1);
-      L.tap_dy[0][r * 3 + s] = static_cast<int8_t>(r - 1);
-    }
+// Where a conv's 3x3 weights land: the one geometry rule behind both the tap tables the kernels read and the weight
+// packer.  Per axis, weight row r of output phase q reads row offset v = q + r - 1, where q is 0 unless the layer folds a
+// nearest-x2 upsample (up / tail write output pixel 2y + q).  Stride 1 reads source pixel y + v.  Every other kind counts
+// v on a grid of twice the resolution its tables address (the stride-2 input, the head's image, the upsampled source),
+// so it reads table offset floor(v / 2), and the parity of v picks the stride-2 parity view, the head's space-to-depth
+// channel group, or (up / tail) which weights merge into one tap.
+struct Slot {
+  int z;           // GEMM phase
+  int tap, dy, dx;
+  int amap;        // activation view: the parity view a stride-2 tap reads
+  int row;         // output-row offset in the GEMM: the tail stacks its four phases in one GEMM
+  int ch;          // input-channel offset in K: the head's space-to-depth parity group
+};
+
+bool folds_upsample(const Layer& L) { return L.kind == K_UP || L.kind == K_TAIL; }
+
+Slot tap_slot(const Layer& L, int qy, int qx, int r, int s) {
+  const int vy = qy + r - 1, vx = qx + s - 1;
+  Slot t{0, r * 3 + s, vy, vx, 0, 0, 0};
+  if (L.kind == K_S1) return t;
+  t.dy = vy >> 1;  // floor(v / 2)
+  t.dx = vx >> 1;
+  const int parity = (vy & 1) * 2 + (vx & 1);
+  if (L.kind == K_S2) {
+    t.amap = parity;
+  } else if (L.kind == K_HEAD) {
+    t.tap = (t.dy + 1) * 2 + (t.dx + 1);
+    t.ch = parity * 16;
+  } else if (L.kind == K_UP) {
+    t.z = qy * 2 + qx;
+    t.tap = (t.dy - qy + 1) * 2 + (t.dx - qx + 1);
+  } else {  // K_TAIL: one GEMM over taps (dy, dx) in {-1,0,1}^2
+    t.row = (qy * 2 + qx) * L.cout;
+    t.tap = (t.dy + 1) * 3 + (t.dx + 1);
+  }
+  return t;
 }
 
-// stride-2, pad-1: input row 2*oy + r - 1 = 2*(oy + d) + parity
-void s2_row(int r, int* parity, int* d) {
-  if (r == 0) { *parity = 1; *d = -1; }
-  else if (r == 1) { *parity = 0; *d = 0; }
-  else { *parity = 1; *d = 0; }
-}
-
-void set_taps_s2(Layer& L) {
-  L.n_phases = 1;
-  L.n_taps = 9;
-  for (int r = 0; r < 3; ++r)
-    for (int s = 0; s < 3; ++s) {
-      int py, dy, px, dx;
-      s2_row(r, &py, &dy);
-      s2_row(s, &px, &dx);
-      L.tap_map[0][r * 3 + s] = static_cast<int8_t>(py * 2 + px);
-      L.tap_dx[0][r * 3 + s] = static_cast<int8_t>(dx);
-      L.tap_dy[0][r * 3 + s] = static_cast<int8_t>(dy);
-    }
-}
-
-// nearest-x2 upsample followed by 3x3 pad-1: output row 2*i + parity reads upsampled rows
-// 2*i + parity + r - 1, i.e. source rows i + d.  Returns d for (parity, r).
-int up_row(int parity, int r) {
-  if (parity == 0) return r == 0 ? -1 : 0;
-  return r == 2 ? 1 : 0;
-}
-
-void set_taps_up(Layer& L) {
-  L.n_phases = 4;
-  L.n_taps = 4;
-  for (int py = 0; py < 2; ++py)
-    for (int px = 0; px < 2; ++px)
-      for (int ty = 0; ty < 2; ++ty)
-        for (int tx = 0; tx < 2; ++tx) {
-          const int z = py * 2 + px, t = ty * 2 + tx;
-          L.tap_map[z][t] = 0;
-          L.tap_dy[z][t] = static_cast<int8_t>(py == 0 ? ty - 1 : ty);
-          L.tap_dx[z][t] = static_cast<int8_t>(px == 0 ? tx - 1 : tx);
+// Tap tables, phase and tap counts, and K (tap-major, then concat source, then channel) of a layer whose kind and
+// sources are set.
+void set_taps(Layer& L) {
+  const int nq = folds_upsample(L) ? 2 : 1;
+  L.n_phases = L.n_taps = 1;
+  for (int qy = 0; qy < nq; ++qy)
+    for (int qx = 0; qx < nq; ++qx)
+      for (int r = 0; r < 3; ++r)
+        for (int s = 0; s < 3; ++s) {
+          const Slot t = tap_slot(L, qy, qx, r, s);
+          L.tap_map[t.z][t.tap] = static_cast<int8_t>(t.amap);
+          L.tap_dy[t.z][t.tap] = static_cast<int8_t>(t.dy);
+          L.tap_dx[t.z][t.tap] = static_cast<int8_t>(t.dx);
+          L.n_phases = std::max(L.n_phases, t.z + 1);
+          L.n_taps = std::max(L.n_taps, t.tap + 1);
         }
-}
-
-void set_taps_head(Layer& L) {
-  L.n_phases = 1;
-  L.n_taps = 4;
-  for (int ty = 0; ty < 2; ++ty)
-    for (int tx = 0; tx < 2; ++tx) {
-      L.tap_map[0][ty * 2 + tx] = 0;
-      L.tap_dy[0][ty * 2 + tx] = static_cast<int8_t>(ty - 1);
-      L.tap_dx[0][ty * 2 + tx] = static_cast<int8_t>(tx - 1);
-    }
-}
-
-void set_taps_tail(Layer& L) {
-  L.n_phases = 1;
-  L.n_taps = 9;
-  for (int ty = 0; ty < 3; ++ty)
-    for (int tx = 0; tx < 3; ++tx) {
-      L.tap_map[0][ty * 3 + tx] = 0;
-      L.tap_dy[0][ty * 3 + tx] = static_cast<int8_t>(ty - 1);
-      L.tap_dx[0][ty * 3 + tx] = static_cast<int8_t>(tx - 1);
-    }
+  L.k_total = L.n_taps * (L.cin[0] + L.cin[1]);
 }
 
 int build_network(lspg_ctx* h) {
@@ -300,7 +282,7 @@ int build_network(lspg_ctx* h) {
     a.kind = K_S1; a.n_src = 1; a.src[0] = x; a.cin[0] = c; a.cout = a.cout_pad = c;
     a.relu = 1; a.has_bn = 1; a.grid_shift = shift;
     a.conv_key = key + ".block.0"; a.bn_key = key + ".block.1";
-    set_taps_s1(a); a.k_total = 9 * c; a.out = new_tensor(c, shift);
+    set_taps(a); a.out = new_tensor(c, shift);
     h->layers.push_back(a);
     Layer b = a;
     b.src[0] = a.out; b.res = x; b.conv_key = key + ".block.3"; b.bn_key = key + ".block.4";
@@ -320,10 +302,11 @@ int build_network(lspg_ctx* h) {
     dn.cout = dn.cout_pad = inner_nc; dn.relu = 1; dn.grid_shift = l + 1;
     dn.conv_key = k.down; dn.bn_key = k.down_bn; dn.has_bn = k.down_bn.empty() ? 0 : 1;
     if (outer) {
-      dn.kind = K_HEAD; dn.n_src = 1; dn.src[0] = s_in; dn.cin[0] = 64; set_taps_head(dn); dn.k_total = 4 * 64;
+      dn.kind = K_HEAD; dn.n_src = 1; dn.src[0] = s_in; dn.cin[0] = 64;
     } else {
-      dn.kind = K_S2; dn.n_src = 1; dn.src[0] = x; dn.cin[0] = outer_nc; set_taps_s2(dn); dn.k_total = 9 * outer_nc;
+      dn.kind = K_S2; dn.n_src = 1; dn.src[0] = x; dn.cin[0] = outer_nc;
     }
+    set_taps(dn);
     dn.out = new_tensor(inner_nc, l + 1);
     h->layers.push_back(dn);
     int e = dn.out;
@@ -336,13 +319,11 @@ int build_network(lspg_ctx* h) {
     up.grid_shift = l + 1;                    // sampling grid = source grid
     up.conv_key = k.up; up.bn_key = k.up_bn; up.has_bn = k.up_bn.empty() ? 0 : 1;
     if (outer) {
-      up.kind = K_TAIL; up.cout = outer_nc; up.cout_pad = 16; up.relu = 0; set_taps_tail(up);
-      up.k_total = 9 * up.n_src * inner_nc; up.out = -1;
+      up.kind = K_TAIL; up.cout = outer_nc; up.cout_pad = 16; up.relu = 0; set_taps(up); up.out = -1;
       h->layers.push_back(up);
       return -1;
     }
-    up.kind = K_UP; up.cout = up.cout_pad = outer_nc; up.relu = 1; set_taps_up(up);
-    up.k_total = 4 * up.n_src * inner_nc; up.out = new_tensor(outer_nc, l);
+    up.kind = K_UP; up.cout = up.cout_pad = outer_nc; up.relu = 1; set_taps(up); up.out = new_tensor(outer_nc, l);
     h->layers.push_back(up);
     int dd = up.out;
     for (const auto& rk : k.res_up) dd = add_res(rk, dd, outer_nc, l);
@@ -352,65 +333,34 @@ int build_network(lspg_ctx* h) {
   return LSPG_OK;
 }
 
+// Input channels of the layer's conv weight: the head reads in_nc image channels, spread over the 64-channel
+// space-to-depth tensor; every other conv reads its concatenated sources.
+int weight_cin(const lspg_ctx* h, const Layer& L) { return L.kind == K_HEAD ? h->in_nc : L.cin[0] + L.cin[1]; }
+
 // ------------------------------------------------------------------------------------------------
 // Weight packing: OIHW fp32 -> [phase][cout_pad][K] (K = tap-major, then concat source, then channel),
 // BatchNorm folded into fp32 scale/shift that the epilogue applies (the weights themselves are NOT scaled,
 // so operand rounding matches "conv then BN").
 // ------------------------------------------------------------------------------------------------
 void pack_layer(lspg_ctx* h, Layer& L) {
-  const int cin_total = (L.kind == K_HEAD) ? h->in_nc : (L.cin[0] + (L.n_src == 2 ? L.cin[1] : 0));
-  const size_t per_phase = static_cast<size_t>(L.cout_pad) * L.k_total;
-  std::vector<float> P(per_phase * L.n_phases, 0.0f);
-  auto W = [&](int o, int c, int r, int s) -> float {
-    return L.w[((static_cast<size_t>(o) * cin_total + c) * 3 + r) * 3 + s];
-  };
-  const int kb_per_tap = (L.cin[0] + (L.n_src == 2 ? L.cin[1] : 0));   // K elements per tap
-  auto kidx = [&](int tap, int c_concat) { return tap * kb_per_tap + c_concat; };
-
-  if (L.kind == K_S1 || L.kind == K_S2) {
-    for (int o = 0; o < L.cout; ++o)
-      for (int r = 0; r < 3; ++r)
-        for (int s = 0; s < 3; ++s)
-          for (int c = 0; c < cin_total; ++c)
-            P[static_cast<size_t>(o) * L.k_total + kidx(r * 3 + s, c)] = W(o, c, r, s);
-  } else if (L.kind == K_UP) {
-    for (int py = 0; py < 2; ++py)
-      for (int px = 0; px < 2; ++px) {
-        float* Pz = P.data() + per_phase * (py * 2 + px);
-        for (int o = 0; o < L.cout; ++o)
-          for (int r = 0; r < 3; ++r)
-            for (int s = 0; s < 3; ++s) {
-              const int ty = up_row(py, r) - (py == 0 ? -1 : 0);   // dy -> tap row index (see set_taps_up)
-              const int tx = up_row(px, s) - (px == 0 ? -1 : 0);
-              for (int c = 0; c < cin_total; ++c)
-                Pz[static_cast<size_t>(o) * L.k_total + kidx(ty * 2 + tx, c)] += W(o, c, r, s);
+  const int cin_w = weight_cin(h, L), nq = folds_upsample(L) ? 2 : 1;
+  const int k_per_tap = L.cin[0] + L.cin[1];
+  std::vector<float> P(static_cast<size_t>(L.n_phases) * L.cout_pad * L.k_total, 0.0f);
+  for (int qy = 0; qy < nq; ++qy)
+    for (int qx = 0; qx < nq; ++qx)
+      for (int o = 0; o < L.cout; ++o)
+        for (int r = 0; r < 3; ++r)
+          for (int s = 0; s < 3; ++s) {
+            const Slot t = tap_slot(L, qy, qx, r, s);
+            float* dst = P.data() + (static_cast<size_t>(t.z) * L.cout_pad + t.row + o) * L.k_total + t.tap * k_per_tap + t.ch;
+            for (int c = 0; c < cin_w; ++c) {
+              const float w = L.w[((static_cast<size_t>(o) * cin_w + c) * 3 + r) * 3 + s];
+              // up / tail: the taps that read one source pixel merge as an fp32 sum from zero, in (r, s) order.  Every
+              // other slot takes its one weight as is (a sum from zero would turn -0.0f into +0.0f).
+              if (nq == 2) dst[c] += w;
+              else dst[c] = w;
             }
-      }
-  } else if (L.kind == K_HEAD) {
-    // source channel (py*2+px)*16 + c of the space-to-depth input, taps (dy,dx) in {-1,0}^2
-    for (int o = 0; o < L.cout; ++o)
-      for (int r = 0; r < 3; ++r)
-        for (int s = 0; s < 3; ++s) {
-          int py, dy, px, dx;
-          s2_row(r, &py, &dy);
-          s2_row(s, &px, &dx);
-          const int tap = (dy + 1) * 2 + (dx + 1);
-          for (int c = 0; c < cin_total; ++c)
-            P[static_cast<size_t>(o) * L.k_total + kidx(tap, (py * 2 + px) * 16 + c)] = W(o, c, r, s);
-        }
-  } else {  // K_TAIL: row n = (py*2+px)*out_nc + c, taps (dy,dx) in {-1,0,1}^2 on the source grid
-    for (int py = 0; py < 2; ++py)
-      for (int px = 0; px < 2; ++px)
-        for (int o = 0; o < L.cout; ++o) {
-          const int n = (py * 2 + px) * L.cout + o;
-          for (int r = 0; r < 3; ++r)
-            for (int s = 0; s < 3; ++s) {
-              const int tap = (up_row(py, r) + 1) * 3 + (up_row(px, s) + 1);
-              for (int c = 0; c < cin_total; ++c)
-                P[static_cast<size_t>(n) * L.k_total + kidx(tap, c)] += W(o, c, r, s);
-            }
-        }
-  }
+          }
   for (int l = 0; l < 3; ++l) L.packed[l].assign(P.size(), 0);
   const float up = static_cast<float>(1 << kParityWeightShift);
   for (size_t i = 0; i < P.size(); ++i) {
@@ -1058,8 +1008,7 @@ int lspg_load_weights(lspg_handle h, const lspg_tensor* tensors, int n) {
   };
   bool synced = false;
   for (auto& L : h->layers) {
-    const int cin_total = (L.kind == K_HEAD) ? h->in_nc : (L.cin[0] + (L.n_src == 2 ? L.cin[1] : 0));
-    const size_t wn = static_cast<size_t>(L.cout) * cin_total * 9;
+    const size_t wn = static_cast<size_t>(L.cout) * weight_cin(h, L) * 9;
     bool changed = false;
     int rc;
     if (L.w.empty()) { L.w.assign(wn, 0.0f); changed = true; }
@@ -1363,10 +1312,9 @@ int lspg_flops_per_frame(lspg_handle h, int height, int width, double* out) {
   double total = 0;
   for (const auto& L : h->layers) {
     // algorithmic work of the REFERENCE conv this layer implements: 2 * Ho*Wo*Cout*Cin*9
-    const int cin_total = (L.kind == K_HEAD) ? h->in_nc : (L.cin[0] + (L.n_src == 2 ? L.cin[1] : 0));
     int oshift = L.grid_shift;                                   // output grid
-    if (L.kind == K_UP || L.kind == K_TAIL) oshift = L.grid_shift - 1;   // upsampled output
-    total += 2.0 * (height >> oshift) * (width >> oshift) * static_cast<double>(L.cout) * cin_total * 9.0;
+    if (folds_upsample(L)) oshift = L.grid_shift - 1;            // upsampled output
+    total += 2.0 * (height >> oshift) * (width >> oshift) * static_cast<double>(L.cout) * weight_cin(h, L) * 9.0;
   }
   *out = total;
   return LSPG_OK;

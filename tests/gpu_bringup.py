@@ -1,17 +1,14 @@
-"""GPU bring-up / bisecting tool (run under gpurun; writes a detailed log).
+"""GPU bring-up tool.
 
     python tests/gpu_bringup.py <stage> [variant] [recipe] [mode] [H] [B]
 
-stage "layers": run one forward with per-layer synchronisation and compare EVERY intermediate activation
-with the CPU plan emulator (tests/plan_emulator.py), printing a per-layer error table and, for the first bad
-layer, the structure of the mismatch (per 64-channel chunk / per tile row / per pixel position).
 stage "final": compare the final image with the oracle.   stage "time": quick timing.
+Per-layer checks of every conv launch are tests/test_gpu_layers.py.
 """
 from __future__ import annotations
 
 import os
 import sys
-import time
 import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
@@ -21,7 +18,6 @@ sys.path.insert(0, HERE)
 import torch  # noqa: E402
 
 from oracle import f2f_oracle as O  # noqa: E402
-import plan_emulator as E  # noqa: E402
 from livespeechportraits_b200.generator import Feature2Face_G  # noqa: E402
 
 
@@ -31,86 +27,6 @@ def make_net(variant, recipe, mode):
     sd = O.make_state_dict(variant, recipe)
     net.load_state_dict(sd, strict=True)
     return net.cuda().eval(), sd
-
-
-def describe_mismatch(got: torch.Tensor, exp: torch.Tensor, tol: float) -> None:
-    # got/exp: [B,H,W,C] float
-    err = (got - exp).abs()
-    bad = err > tol
-    print(f"    bad fraction {bad.float().mean().item():.4f}; got std {got.std().item():.4f} exp std {exp.std().item():.4f}"
-          f" got nan {torch.isnan(got).sum().item()}")
-    b, h, w, c = got.shape
-    for c0 in range(0, c, 64):
-        e = err[..., c0:c0 + 64]
-        print(f"    channels {c0:4d}..{c0 + 63:4d}: max {e.max().item():.4g} mean {e.mean().item():.4g}")
-        if c0 >= 192:
-            break
-    pe = err.amax(dim=3)[0]                      # [H,W] of image 0
-    rows = pe.amax(dim=1)
-    cols = pe.amax(dim=0)
-    print("    per-row max err (first 24 rows):", [f"{v:.2g}" for v in rows[:24].tolist()])
-    print("    per-col max err (first 24 cols):", [f"{v:.2g}" for v in cols[:24].tolist()])
-    ce = err.amax(dim=(0, 1, 2))
-    print("    per-channel max err (first 32):", [f"{v:.2g}" for v in ce[:32].tolist()])
-    print("    sample got[0,0,0,:8]", [f"{v:.4f}" for v in got[0, 0, 0, :8].tolist()])
-    print("    sample exp[0,0,0,:8]", [f"{v:.4f}" for v in exp[0, 0, 0, :8].tolist()])
-    print("    sample got[0,5,7,:8]", [f"{v:.4f}" for v in got[0, min(5, h - 1), min(7, w - 1), :8].tolist()])
-    print("    sample exp[0,5,7,:8]", [f"{v:.4f}" for v in exp[0, min(5, h - 1), min(7, w - 1), :8].tolist()])
-
-
-def stage_layers(variant, recipe, mode, H, B):
-    os.environ["LSPG_DEBUG_SYNC"] = "1"
-    net, sd = make_net(variant, recipe, mode)
-    fm, cand = O.make_inputs(B, H, H)
-    x = torch.cat([fm, cand], 1)
-    limbs = 2 if mode == "parity" else 1
-    rnd = (lambda t: t) if mode == "parity" else (lambda t: t.bfloat16().float())
-    plan = E.HostPlan(variant, sd)
-    taps = {}
-    t0 = time.time()
-    exp_out = E.run_plan(plan, x, limbs=limbs, round_act=rnd, taps_out=taps)
-    print(f"emulator done in {time.time() - t0:.1f}s", flush=True)
-    try:
-        out = net(x.cuda())
-        torch.cuda.synchronize()
-    except Exception as e:  # noqa: BLE001
-        print("FORWARD FAILED:", e, flush=True)
-        return 1
-    print("forward returned", flush=True)
-    # input packer
-    first_bad = None
-
-    def read(tid):
-        t = net.debug_read_tensor(tid, B, H, H, 0).float()
-        if mode == "parity":
-            t = t + net.debug_read_tensor(tid, B, H, H, 1).float()
-        return t
-    got0 = read(0)
-    exp0 = rnd(E.pack_input_s2d(x))
-    print(f"tensor 0 (packed input): max err {(got0 - exp0).abs().max().item():.3g}")
-    for i, L in enumerate(plan.layers):
-        if L.out < 0:
-            continue
-        got = read(L.out)
-        exp = taps[L.out]
-        scale = max(exp.abs().max().item(), 1e-6)
-        err = (got - exp).abs().max().item()
-        tol = 0.02 * scale + 1e-3 if mode != "parity" else 2e-3 * scale + 1e-4
-        flag = "ok " if err <= tol else "BAD"
-        print(f"layer {i:2d} kind {L.kind} {L.conv_key.decode():44s} out t{L.out:<3d} {tuple(got.shape)} max|exp| {scale:8.4f} "
-              f"err {err:9.4g} {flag}", flush=True)
-        if err > tol and first_bad is None:
-            first_bad = i
-            describe_mismatch(got, exp, tol)
-    o = out.float().cpu()
-    err = (o - exp_out).abs().max().item()
-    print(f"final image: max err vs emulator {err:.4g}; vs oracle "
-          f"{(o - O.generator_forward(sd, x, variant)).abs().max().item():.4g}", flush=True)
-    if first_bad is None and err > 0.05:
-        y = o.permute(0, 2, 3, 1)
-        e = exp_out.permute(0, 2, 3, 1)
-        describe_mismatch(y, e, 0.01)
-    return 0 if first_bad is None else 2
 
 
 def stage_final(variant, recipe, mode, H, B):
@@ -167,4 +83,4 @@ if __name__ == "__main__":
     H = int(sys.argv[5]) if len(sys.argv) > 5 else 256
     B = int(sys.argv[6]) if len(sys.argv) > 6 else 1
     print(f"=== {stage} {variant} {recipe} {mode} H={H} B={B} on {torch.cuda.get_device_name(0)}", flush=True)
-    sys.exit({"layers": stage_layers, "final": stage_final, "time": stage_time}[stage](variant, recipe, mode, H, B))
+    sys.exit({"final": stage_final, "time": stage_time}[stage](variant, recipe, mode, H, B))

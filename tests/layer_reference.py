@@ -1,8 +1,9 @@
 """Float64 reference of one conv launch of the generator, and the per-element error bound its CUDA kernel must meet.
 
 The layer's meaning comes from the state dict and the layer kind only (conv_key / bn_key / src / res / relu of an
-``LspgLayerInfo`` row); nothing is read from the library's tap tables or packed weights, so a geometry or packing bug
-cannot hide in both the kernel and this reference.
+``LspgLayerInfo`` row); the reference reads nothing from the library's tap tables or packed weights, so a geometry or
+packing bug cannot hide in both the kernel and this reference.  ``Net`` reads those back from a host-only handle for the
+tests that compare them with the reference.
 
 Every layer is written as a sum over *groups*: one source-grid offset (dy, dx) times one 64-channel chunk of the
 concatenated sources.  For a stride-1/2 conv the offsets are the 3x3 taps; for nearest-x2 upsample + conv and for the
@@ -16,10 +17,14 @@ Quantities are float64 torch tensors on any device; activations are NHWC.
 """
 from __future__ import annotations
 
+import ctypes as C
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
+import numpy as np
 import torch
+
+from livespeechportraits_b200 import _lib
 
 KIND_HEAD, KIND_S1, KIND_S2, KIND_UP, KIND_TAIL = range(5)
 BN_EPS = 1e-5
@@ -322,10 +327,55 @@ def pack_s2d(x: torch.Tensor) -> torch.Tensor:
     return s
 
 
+class Net:
+    """Host-only library handle (no device): the layer rows, the planner's geometry at 132 SMs and, once a state dict
+    is loaded, the packed weights and folded BatchNorm.  These are what the tests compare the reference against."""
+
+    def __init__(self, variant: str, sd: Optional[Dict[str, torch.Tensor]] = None):
+        self.lib = _lib.load()
+        self.h = C.c_void_p()
+        _lib.check(self.lib.lspg_create(C.byref(self.h), _lib.LSPG_VARIANT[variant], 64, 8, 13, 3, -1))
+        n = C.c_int()
+        _lib.check(self.lib.lspg_num_layers(self.h, C.byref(n)))
+        self.layers = []
+        for i in range(n.value):
+            info = _lib.LspgLayerInfo()
+            _lib.check(self.lib.lspg_layer_info_get(self.h, i, C.byref(info)))
+            self.layers.append(info)
+        if sd is not None:
+            keep = [(k.encode(), v.float().contiguous()) for k, v in sd.items() if not k.endswith("num_batches_tracked")]
+            arr = (_lib.LspgTensor * len(keep))()
+            for i, (k, t) in enumerate(keep):
+                arr[i].name, arr[i].numel, arr[i].data = k, t.numel(), C.cast(t.data_ptr(), C.POINTER(C.c_float))
+            _lib.check(self.lib.lspg_load_weights(self.h, arr, len(keep)))
+
+    def geo(self, i, b, hh, ww):
+        g = _lib.LspgLayerGeo()
+        _lib.check(self.lib.lspg_debug_layer_geo(self.h, i, b, hh, ww, C.byref(g)))
+        return g
+
+    def packed(self, i: int, limb: int) -> np.ndarray:
+        """Raw 16-bit words of packed limb ``limb`` of layer i (0/1: PARITY fp16 hi/lo of w * 2^8, 2: FAST bf16),
+        [phase][cout_pad][K] flattened."""
+        info = self.layers[i]
+        count = info.n_phases * info.cout_pad * info.k_total
+        buf = np.zeros(count, np.uint16)
+        _lib.check(self.lib.lspg_layer_packed(self.h, i, limb, buf.ctypes.data, count))
+        return buf
+
+    def affine(self, i: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The folded BatchNorm (scale, shift) the epilogue applies, [cout_pad] fp32 each."""
+        n = self.layers[i].cout_pad
+        s, b = np.zeros(n, np.float32), np.zeros(n, np.float32)
+        _lib.check(self.lib.lspg_layer_affine(self.h, i, s.ctypes.data, b.ctypes.data, n))
+        return torch.from_numpy(s), torch.from_numpy(b)
+
+    def close(self):
+        self.lib.lspg_destroy(self.h)
+
+
 def planner_variants(lib, handle, batch: int, height: int, width: int) -> Dict[tuple, List[int]]:
     """(kernel, BN, tail, cluster, split-K) -> layers the planner gives it for this problem size."""
-    import ctypes as C
-    from livespeechportraits_b200 import _lib
     n = C.c_int()
     _lib.check(lib.lspg_num_layers(handle, C.byref(n)))
     out: Dict[tuple, List[int]] = {}

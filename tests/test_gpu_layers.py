@@ -35,17 +35,6 @@ def variant_key(info, g) -> tuple:
     return ("patch" if g.kernel == 1 else "umma", g.bn, info.kind == R.KIND_TAIL, g.cluster, g.n_split > 1)
 
 
-def _host_variants(variant, batch, hh, ww):
-    from livespeechportraits_b200 import _lib
-    lib = _lib.load()
-    h = C.c_void_p()
-    _lib.check(lib.lspg_create(C.byref(h), _lib.LSPG_VARIANT[variant], 64, 8, 13, 3, -1))
-    try:
-        return set(R.planner_variants(lib, h, batch, hh, ww))
-    finally:
-        lib.lspg_destroy(h)
-
-
 def _ulp_f16(hi: torch.Tensor) -> torch.Tensor:
     a = hi.float().abs()
     _, e = torch.frexp(a)                                  # a = m * 2^e, m in [0.5, 1)
@@ -53,7 +42,7 @@ def _ulp_f16(hi: torch.Tensor) -> torch.Tensor:
     return torch.where(a == 0, torch.full_like(a, 2.0 ** -24), ulp)
 
 
-def _run_config(variant, recipe, batch, hh, ww, mode):
+def _run_config(variant, recipe, batch, hh, ww, mode, layers):
     from livespeechportraits_b200 import _lib
     from livespeechportraits_b200.generator import Feature2Face_G
     opt = types.SimpleNamespace(isTrain=False, size=variant, n_downsample_G=8, ngf=64, fp16=0)
@@ -96,13 +85,9 @@ def _run_config(variant, recipe, batch, hh, ww, mode):
     for q in range(4):
         assert all((t[..., q * 16 + 13:q * 16 + 16] == 0).all() for t in tensors[0]), "space-to-depth pad channels must be zero"
 
-    nl = C.c_int()
-    _lib.check(lib.lspg_num_layers(h, C.byref(nl)))
     worst = {}                                        # (variant key, tier) -> (err/bound, layer, conv key)
     failures = []
-    for i in range(nl.value):
-        info = _lib.LspgLayerInfo()
-        _lib.check(lib.lspg_layer_info_get(h, i, C.byref(info)))
+    for i, info in enumerate(layers):
         g = _lib.LspgLayerGeo()
         _lib.check(lib.lspg_debug_layer_geo(h, i, batch, hh, ww, C.byref(g)))
         key = variant_key(info, g)
@@ -131,7 +116,7 @@ def _run_config(variant, recipe, batch, hh, ww, mode):
                                 f"bound {bnd[n, y, xq, c].item():.3g}; " + _where(info, g, xin[0].shape, n, y, xq, c, sms))
         del sem_v, sem_b, ker_v, ker_b
         for tid in list(tensors):                     # keep only what later layers read
-            if tid != 0 and tid not in _later_reads(lib, h, i, nl.value):
+            if tid != 0 and tid not in _later_reads(layers, i):
                 del tensors[tid]
     # fused tensor2im of the same run
     img = net.render_image(x.cuda(), None).cpu().numpy()
@@ -156,12 +141,9 @@ def _where(info, g, src_shape, n, y, x, c, sms) -> str:
             f"{t // ctas}, {'odd' if (t // ctas) % 2 else 'even'}{', split 0' if g.n_split > 1 else ''})")
 
 
-def _later_reads(lib, h, i, n):
-    from livespeechportraits_b200 import _lib
+def _later_reads(layers, i):
     ids = set()
-    for j in range(i + 1, n):
-        info = _lib.LspgLayerInfo()
-        lib.lspg_layer_info_get(h, j, C.byref(info))
+    for info in layers[i + 1:]:
         ids.update(info.src[s] for s in range(info.n_src))
         if info.res >= 0:
             ids.add(info.res)
@@ -171,11 +153,16 @@ def _later_reads(lib, h, i, n):
 @pytest.mark.parametrize("mode", ["parity", "fast"])
 @pytest.mark.parametrize("cfg", GPU_LAYER_CONFIGS, ids=lambda c: f"{c[0]}{c[1]}_b{c[2]}_{c[3]}x{c[4]}")
 def test_every_layer_against_float64_reference(cfg, mode):
-    worst, sms, failures = _run_config(*cfg, mode)
+    host = R.Net(cfg[0])                              # layer rows, and the variants the planner picks at 132 SMs
+    try:
+        worst, sms, failures = _run_config(*cfg, mode, host.layers)
+        reachable = set(R.planner_variants(host.lib, host.h, *cfg[2:]))
+    finally:
+        host.close()
     for key, tier in sorted(worst):
         r, i, k = worst[(key, tier)]
         print(f"[layers] {cfg} {mode} {key} {tier}: worst err/bound {r:.3g} (layer {i} {k})")
-    missed = _host_variants(*[cfg[0]] + list(cfg[2:])) - {key for key, _ in worst}
+    missed = reachable - {key for key, _ in worst}
     if missed:
         print(f"[layers] device has {sms} SMs: variants this config reaches at 132 SMs that did not run: {sorted(missed)}")
     assert not failures, "\n".join(failures[:8])

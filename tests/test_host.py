@@ -1,19 +1,19 @@
-"""Host-side logic, CPU only: the C ABI loads and exports what include/lspg.h declares, error behaviour,
-the drop-in module's state-dict contract, and the launch plan (structure, packing, BatchNorm folding, tap
-geometry) executed by the CPU plan emulator against the oracle.  No GPU compute here."""
+"""Host-side logic, CPU only: the C ABI loads and exports what include/lspg.h declares, error behaviour, the drop-in
+module's state-dict contract, the BatchNorm fold, FLOP accounting and the launch planner.  The layer list, tap tables
+and packed weights are pinned exactly against the per-layer reference in tests/test_layer_reference.py.  No GPU compute
+here."""
 import ctypes as C
 import os
 import re
 import types
 
-import numpy as np
 import pytest
 import torch
 
 from livespeechportraits_b200 import _lib
 from livespeechportraits_b200.generator import Feature2Face_G
 from oracle import f2f_oracle as O
-import plan_emulator as E
+import layer_reference as R
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -101,32 +101,12 @@ def test_module_refuses_cpu_and_train_mode():
         Feature2Face_G(opt("small"))
 
 
-@pytest.mark.parametrize("variant,recipe", [("normal", "B"), ("large", "A")])
-def test_launch_plan_reproduces_the_oracle(variant, recipe):
-    sd = O.make_state_dict(variant, recipe)
-    plan = E.HostPlan(variant, sd)
-    try:
-        kinds = [L.kind for L in plan.layers]
-        assert kinds[0] == E.KIND_HEAD and kinds[-1] == E.KIND_TAIL
-        assert len(kinds) == (76 if variant == "large" else 46)
-        fm, cand = O.make_inputs(1, 256, 256)
-        x = torch.cat([fm, cand], 1)
-        ref = O.generator_forward(sd, x, variant)
-        out = E.run_plan(plan, x, limbs=2)
-        # hi+lo fp16 weights carry 22 mantissa bits: the plan (fp32 activations here) must reproduce the oracle to ~1e-4
-        assert (out - ref).abs().max().item() <= 2e-4
-        out_bf16 = E.run_plan(plan, x, limbs=1, round_act=lambda t: t.bfloat16().float())
-        assert (out_bf16 - ref).abs().max().item() <= 5e-2
-    finally:
-        plan.close()
-
-
 def test_bn_fold_matches_batchnorm_formula():
     sd = O.make_state_dict("normal", "B")
-    plan = E.HostPlan("normal", sd)
+    net = R.Net("normal", sd)
     try:
-        for i, L in enumerate(plan.layers):
-            s, b = plan.affine(i)
+        for i, L in enumerate(net.layers):
+            s, b = net.affine(i)
             if L.has_bn:
                 key = L.bn_key.decode()
                 inv = 1.0 / torch.sqrt(sd[key + ".running_var"] + 1e-5)
@@ -136,7 +116,7 @@ def test_bn_fold_matches_batchnorm_formula():
             else:
                 assert float((s - 1).abs().max()) == 0 and float(b.abs().max()) == 0
     finally:
-        plan.close()
+        net.close()
 
 
 def test_flops_accounting_matches_oracle():
@@ -200,21 +180,13 @@ def test_tile_decode_division_by_multiply_high_is_exact():
 
 
 def _geo_table(variant, batch, height=512, width=512):
-    lib = _lib.load()
-    h = C.c_void_p()
-    assert lib.lspg_create(C.byref(h), _lib.LSPG_VARIANT[variant], 64, 8, 13, 3, -1) == 0
-    n = C.c_int()
-    assert lib.lspg_num_layers(h, C.byref(n)) == 0
-    out = []
-    for i in range(n.value):
-        g = _lib.LspgLayerGeo()
-        assert lib.lspg_debug_layer_geo(h, i, batch, height, width, C.byref(g)) == 0
-        info = _lib.LspgLayerInfo()
-        assert lib.lspg_layer_info_get(h, i, C.byref(info)) == 0
-        out.append((info, g))
-    need = C.c_size_t()
-    assert lib.lspg_workspace_bytes(h, batch, height, width, 1, C.byref(need)) == 0
-    lib.lspg_destroy(h)
+    net = R.Net(variant)
+    try:
+        out = [(info, net.geo(i, batch, height, width)) for i, info in enumerate(net.layers)]
+        need = C.c_size_t()
+        assert net.lib.lspg_workspace_bytes(net.h, batch, height, width, 1, C.byref(need)) == 0
+    finally:
+        net.close()
     return out, need.value
 
 

@@ -2,6 +2,8 @@
 configurations the GPU per-layer test runs (tests/test_gpu_layers.py).
 
 * The reference is right: chained over the network it reproduces the float64 oracle.
+* The library's tap tables and packed weights (both PARITY limbs and the FAST bf16) are exactly what the reference
+  derives from the state dict.
 * The bound is right and has teeth: a float64 emulation of the kernels' arithmetic (operand limbs, fp32 accumulator
   rounded after every k16 MMA in the kernel's K order, split-K partials, fp32 epilogue, 16-bit stores) passes it at
   every layer, and six small defects of that arithmetic each fail it at some layer.
@@ -9,7 +11,6 @@ configurations the GPU per-layer test runs (tests/test_gpu_layers.py).
 """
 from __future__ import annotations
 
-import ctypes as C
 import os
 import sys
 
@@ -24,36 +25,6 @@ from livespeechportraits_b200 import _lib  # noqa: E402
 
 CPU_CONFIGS = [("normal", "B"), ("large", "A")]       # at 256 x 256, one frame
 HW = 256
-
-
-class Net:
-    """Host-only handle: layer rows and the planner's geometry at 132 SMs."""
-
-    def __init__(self, variant, sd=None):
-        self.lib = _lib.load()
-        self.h = C.c_void_p()
-        _lib.check(self.lib.lspg_create(C.byref(self.h), _lib.LSPG_VARIANT[variant], 64, 8, 13, 3, -1))
-        n = C.c_int()
-        _lib.check(self.lib.lspg_num_layers(self.h, C.byref(n)))
-        self.layers = []
-        for i in range(n.value):
-            info = _lib.LspgLayerInfo()
-            _lib.check(self.lib.lspg_layer_info_get(self.h, i, C.byref(info)))
-            self.layers.append(info)
-        if sd is not None:
-            keep = [(k.encode(), v.float().contiguous()) for k, v in sd.items() if not k.endswith("num_batches_tracked")]
-            arr = (_lib.LspgTensor * len(keep))()
-            for i, (k, t) in enumerate(keep):
-                arr[i].name, arr[i].numel, arr[i].data = k, t.numel(), C.cast(t.data_ptr(), C.POINTER(C.c_float))
-            _lib.check(self.lib.lspg_load_weights(self.h, arr, len(keep)))
-
-    def geo(self, i, b, hh, ww):
-        g = _lib.LspgLayerGeo()
-        _lib.check(self.lib.lspg_debug_layer_geo(self.h, i, b, hh, ww, C.byref(g)))
-        return g
-
-    def close(self):
-        self.lib.lspg_destroy(self.h)
 
 
 def _store(v: torch.Tensor, mode: str):
@@ -88,7 +59,7 @@ def _chain(sd, net, x, mode):
 def chained(request):
     variant, recipe = request.param
     sd = O.make_state_dict(variant, recipe)
-    net = Net(variant, sd)
+    net = R.Net(variant, sd)
     fm, cand = O.make_inputs(1, HW, HW)
     x = torch.cat([fm, cand], 1)
     yield variant, recipe, sd, net, x
@@ -99,6 +70,9 @@ def test_reference_chain_matches_float64_oracle(chained):
     """Chaining the per-layer reference reproduces the oracle (pinned bit-exact against the reference module) run on a
     float64 copy of the state dict, to float64 rounding."""
     variant, _, sd, net, x = chained
+    kinds = [info.kind for info in net.layers]
+    assert len(kinds) == (76 if variant == "large" else 46)
+    assert kinds[0] == R.KIND_HEAD and kinds[-1] == R.KIND_TAIL
     sd64 = {k: (v.double() if v.is_floating_point() else v) for k, v in sd.items()}
     want = O.generator_forward(sd64, x.double(), variant)
     _, got = _chain(sd, net, x, None)
@@ -107,23 +81,35 @@ def test_reference_chain_matches_float64_oracle(chained):
 
 
 def test_fast_weights_match_packed(chained):
-    """The bf16 weights the FAST reference multiplies, built from the state dict, equal what the library packed (limb 2),
-    so a packing error reports here and not as a kernel error."""
+    """The library's tap tables and packed weights equal, bit for bit, what the reference builds from the state dict and
+    the layer kind: the (dy, dx, parity view) of every tap, the PARITY hi / lo limbs of w * 2^8 (limbs 0 and 1) and the
+    FAST bf16 weights (limb 2), in the [phase][cout][tap][channel] layout with zeros everywhere else.  So a geometry or
+    packing error reports here and not as a kernel error."""
     _, _, sd, net, _ = chained
     for i, info in enumerate(net.layers):
         spec = R.layer_spec(sd, info, "fast")
-        count = info.n_phases * info.cout_pad * info.k_total
-        buf = np.zeros(count, np.uint16)
-        _lib.check(net.lib.lspg_layer_packed(net.h, i, 2, buf.ctypes.data, count))
-        packed = torch.from_numpy((buf.astype(np.uint32) << 16).view(np.float32).copy()).double()
-        packed = packed.view(info.n_phases, info.cout_pad, -1, spec.cin)          # [phase][cout][tap][channel]
+        tail = info.kind == R.KIND_TAIL              # one GEMM: columns (phase, channel), taps (dy, dx) in {-1,0,1}^2
+        assert info.n_phases == (1 if tail else len(spec.phases)), (i, info.n_phases)
+        assert info.n_taps == (9 if tail else len(spec.offsets[0])) and info.k_total == info.n_taps * spec.cin, i
+        got = [torch.from_numpy(net.packed(i, limb).view(np.int16)).view(info.n_phases, info.cout_pad, info.n_taps, spec.cin)
+               for limb in range(3)]
+        want = [torch.zeros_like(g) for g in got]
         for z in range(len(spec.phases)):
             for t, off in enumerate(spec.offsets[z]):
-                if info.kind == R.KIND_TAIL:          # one GEMM: columns (phase, channel), taps (dy, dx) in {-1,0,1}^2
-                    got = packed[0, z * spec.cout:(z + 1) * spec.cout, (off[0] + 1) * 3 + off[1] + 1].t()
+                zt, rows = (0, slice(z * spec.cout, (z + 1) * spec.cout)) if tail else (z, slice(0, spec.cout))
+                if tail:
+                    t = (off[0] + 1) * 3 + off[1] + 1
+                dy, dx, amap = int(info.tap_dy[zt][t]), int(info.tap_dx[zt][t]), int(info.tap_map[zt][t])
+                if info.kind == R.KIND_S2:
+                    assert (2 * dy + (amap >> 1), 2 * dx + (amap & 1)) == off, (i, info.conv_key, z, t)
                 else:
-                    got = packed[z, :spec.cout, t].t()
-                assert torch.equal(got, spec.w[z][off]), (i, info.conv_key, z, off)
+                    assert (dy, dx, amap) == (*off, 0), (i, info.conv_key, z, t)
+                hi, lo = R.kernel_weights(spec, z, off, slice(None), "parity")
+                want[0][zt, rows, t] = hi.t().half().view(torch.int16)
+                want[1][zt, rows, t] = lo.t().half().view(torch.int16)
+                want[2][zt, rows, t] = spec.w[z][off].t().bfloat16().view(torch.int16)
+        for limb in range(3):
+            assert torch.equal(got[limb], want[limb]), (i, info.conv_key, "limb", limb)
 
 
 def _tile_pixels(g, t, batch, hs, ws):
@@ -275,7 +261,7 @@ def test_gpu_configs_cover_every_planner_variant():
     from test_gpu_layers import GPU_LAYER_CONFIGS
     reachable, covered = {}, set()
     for variant in ("normal", "large"):
-        net = Net(variant)
+        net = R.Net(variant)
         for hh, ww in SWEEP_SHAPES:
             for b in SWEEP_BATCHES:
                 for key in R.planner_variants(net.lib, net.h, b, hh, ww):
