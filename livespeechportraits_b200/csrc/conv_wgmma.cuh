@@ -18,7 +18,10 @@
 //     eval-BatchNorm scale/shift in fp32, residual, ReLU, 16-bit (hi, lo) NHWC stores.  The tail variant (patch kernel
 //     only) applies tanh and scatters fp32 NCHW or uint8 HWC directly.
 //     conv_umma_kernel: consumer w owns rows [64w, 64w+64) of every tile.  conv_patch_kernel: ping-pong, consumer w
-//     owns every other tile (all 128 rows, two accumulators), so its epilogue runs under the other one's MMAs.
+//     owns every other tile (all 128 rows, two accumulators), so its epilogue runs under the other one's MMAs.  At
+//     BN = 64 (not the tail) conv_patch_kernel swaps the operand roles: D^T[64 channels x 128 pixels] = W * X^T is one
+//     wgmma.m64n128k16 per limb product, and its epilogue (epilogue_cols) stages the tile in shared memory to write
+//     whole 128-byte channel rows with 16-byte stores.
 //   * NL = 2 ("parity" precision): activations and weights are split into fp16 hi + lo limbs; each K step issues
 //     hi*hi + hi*lo + lo*hi into one accumulator (22 mantissa bits per operand, fp32 accumulate) and the epilogue writes
 //     both limbs.  NL = 1 ("fast"): one bf16 limb, one MMA per K step.
@@ -108,14 +111,15 @@ struct alignas(64) ConvParams {
   CUtensorMap w;             // packed weights, dims {K, Cout_pad, limb*n_phases + phase} (patch kernel: {kc, Cout, tap, limb*phase})
 };
 
-// Shared-memory regions after the operand rings: barriers, then (patch kernel, tail) the accumulator staging of the tail
-// epilogue, one tile per consumer warpgroup (its consumers own whole tiles).
+// Shared-memory regions after the operand rings: barriers, then (patch kernel) the epilogue staging of each consumer
+// warpgroup (its consumers own whole tiles): the tail's 128 accumulator rows, or 64 pixels of a BN = 64 tile.
 constexpr int kBarBytes = 1024;
 constexpr int kTailStride = 17;                                      // floats per staged tail row (16 + 1: no bank conflicts)
-template <bool TAIL>
+constexpr int kColStride = 68;                                       // floats per staged BN = 64 pixel (see epilogue_cols)
+template <int BN, bool TAIL>
 struct AuxCfg {
-  static constexpr int kTailBytes = TAIL ? 2 * kTileM * kTailStride * 4 : 0;
-  static constexpr int kBytes = kBarBytes + kTailBytes;
+  static constexpr int kStgBytes = TAIL ? 2 * kTileM * kTailStride * 4 : (BN == 64 ? 2 * 64 * kColStride * 4 : 0);
+  static constexpr int kBytes = kBarBytes + kStgBytes;
 };
 
 template <int BN, int NL>
@@ -226,14 +230,11 @@ __device__ __forceinline__ __nv_bfloat16* out_pixel(const ConvParams& p, const T
   return p.out_ptr + ((static_cast<size_t>(n) * oh + oy) * ow + ox) * p.out_channels;
 }
 
-// Regular epilogue of channel pair j of a pixel, whose channels start at out[kStride * j] (limb 0) and, in PARITY, at
-// out[out_limb_stride + kStride * j]: folded BatchNorm fma, the residual's limbs in limb order (rw[l][j] = the pair's
-// word of limb l, read only if p.has_res), ReLU, then the 16-bit hi word and the lo word of the remainder y - hi.
-template <int kStride, int NL, int M>
-__device__ __forceinline__ void epilogue_pair(const ConvParams& p, float a0, float a1, float2 s2, float2 f2,
-                                              const uint32_t (&rw)[NL][M], int j, __nv_bfloat16* out) {
-  float y0 = fmaf(a0, s2.x, f2.x);
-  float y1 = fmaf(a1, s2.y, f2.y);
+// Rest of the regular epilogue of channel pair j after the folded BatchNorm fma (y0, y1): the residual's limbs in limb
+// order (rw[l][j] = the pair's word of limb l, read only if p.has_res), ReLU, then the 16-bit hi word (.x) and, in
+// PARITY, the lo word of the remainder y - hi (.y).
+template <int NL, int M>
+__device__ __forceinline__ uint2 finish_pair(const ConvParams& p, float y0, float y1, const uint32_t (&rw)[NL][M], int j) {
   if (p.has_res) {
 #pragma unroll
     for (int l = 0; l < NL; ++l) {
@@ -243,9 +244,17 @@ __device__ __forceinline__ void epilogue_pair(const ConvParams& p, float a0, flo
   }
   if (p.relu) { y0 = fmaxf(y0, 0.0f); y1 = fmaxf(y1, 0.0f); }
   const uint32_t o = pack2<NL == 2>(y0, y1);
-  *reinterpret_cast<uint32_t*>(out + kStride * j) = o;
-  if (NL == 2)
-    *reinterpret_cast<uint32_t*>(out + p.out_limb_stride + kStride * j) = pack2<true>(y0 - unpack_lo<true>(o), y1 - unpack_hi<true>(o));
+  return make_uint2(o, NL == 2 ? pack2<true>(y0 - unpack_lo<true>(o), y1 - unpack_hi<true>(o)) : 0u);
+}
+
+// Regular epilogue of channel pair j of a pixel, whose channels start at out[kStride * j] (limb 0) and, in PARITY, at
+// out[out_limb_stride + kStride * j]: folded BatchNorm fma, then finish_pair.
+template <int kStride, int NL, int M>
+__device__ __forceinline__ void epilogue_pair(const ConvParams& p, float a0, float a1, float2 s2, float2 f2,
+                                              const uint32_t (&rw)[NL][M], int j, __nv_bfloat16* out) {
+  const uint2 o = finish_pair<NL>(p, fmaf(a0, s2.x, f2.x), fmaf(a1, s2.y, f2.y), rw, j);
+  *reinterpret_cast<uint32_t*>(out + kStride * j) = o.x;
+  if (NL == 2) *reinterpret_cast<uint32_t*>(out + p.out_limb_stride + kStride * j) = o.y;
 }
 
 // Consumer epilogue of the 64 tile rows [rb, rb+64) held by one m64nBN accumulator of the calling warpgroup.
@@ -355,6 +364,93 @@ __device__ __forceinline__ void epilogue_regs(const ConvParams& p, const float (
         const float2 f2 = __ldg(reinterpret_cast<const float2*>(sf + 8 * j));
         epilogue_pair<8>(p, acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], s2, f2, rw, j, out_row);
       }
+    }
+  }
+}
+
+// Epilogue of a transposed BN = 64 tile of the patch kernel: acc = D^T[64 channels x 128 tile rows] of one m64n128
+// accumulator (thread layout as in epilogue_regs: channels r0 = 16*warp + lane/4 and r0 + 8, tile rows 8j + 2*(lane%4)
+// and +1).  The folded BatchNorm fma runs in registers (split-K: the raw sums), then each 64-row half goes through the
+// calling warpgroup's staging `stg` (named barrier `bar`) to [row][channel], and a thread finishes 8 channels of a pixel
+// at a time: 16-byte residual loads and output stores, one pixel's 128 contiguous bytes per limb from 8 threads.
+// Staging: row stride kColStride = 68 floats (the 4 rows of one store instruction land 4 banks apart), and channels
+// 32..63 are stored with the two 4-channel halves of each 8-channel chunk swapped, so that the 8 threads of a quarter
+// warp read one pixel's chunks on 32 distinct banks.
+template <int NL>
+__device__ __forceinline__ void epilogue_cols(const ConvParams& p, const float (&acc)[64], const TileCoord& tc, int t,
+                                              float* stg, int bar) {
+  const int wtid = threadIdx.x & 127;
+  const int warp = wtid >> 5, lane = wtid & 31;
+  const int r0 = warp * 16 + (lane >> 2);
+  const int c0 = 2 * (lane & 3);
+  const bool raw = p.n_split > 1;
+  float sc[2] = {1.0f, 1.0f}, sf[2] = {0.0f, 0.0f};
+  if (!raw) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      sc[h] = __ldg(p.scale + tc.nt * 64 + r0 + 8 * h);
+      sf[h] = __ldg(p.shift + tc.nt * 64 + r0 + 8 * h);
+    }
+  }
+  float* const st_w = stg + c0 * kColStride + (r0 ^ ((warp & 2) << 1));   // channel r0 (+8 for r0 + 8) of row c0
+  const int k = wtid & 7;                                                 // reader: channels [8k, 8k + 8) ...
+  const int kb = k >> 2;                                                  // ... whose first half is stored second if k >= 4
+  const int ch = tc.nt * 64 + 8 * k;
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    // reader rows 64hh + wtid/8 + 16i: their addresses and residual words first (the loads are in flight during staging)
+    __nv_bfloat16* out[4];
+    uint32_t rw[4][NL][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      int pn, py_, px_;
+      row_pixel(p, tc, 64 * hh + (wtid >> 3) + 16 * i, pn, py_, px_);
+      out[i] = nullptr;
+      if (pn >= p.batch || py_ >= p.hs || px_ >= p.ws) continue;
+      out[i] = out_pixel(p, tc, pn, py_, px_) + ch;
+      if (!raw && p.has_res) {
+        const __nv_bfloat16* res = p.res_ptr + ((static_cast<size_t>(pn) * p.hs + py_) * p.ws + px_) * p.res_channels + ch;
+#pragma unroll
+        for (int l = 0; l < NL; ++l) {
+          const uint4 r = __ldg(reinterpret_cast<const uint4*>(res + l * p.res_limb_stride));
+          rw[i][l][0] = r.x; rw[i][l][1] = r.y; rw[i][l][2] = r.z; rw[i][l][3] = r.w;
+        }
+      }
+    }
+    ptx::named_bar_sync(bar, 128);                        // the previous half's rows have been read
+#pragma unroll
+    for (int j = 0; j < 8; ++j)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const float a = acc[4 * (8 * hh + j) + 2 * h + e];
+          st_w[(8 * j + e) * kColStride + 8 * h] = raw ? a : fmaf(a, sc[h], sf[h]);
+        }
+    ptx::named_bar_sync(bar, 128);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if (out[i] == nullptr) continue;
+      const int row = 64 * hh + (wtid >> 3) + 16 * i;
+      const float* src = stg + (row - 64 * hh) * kColStride + 8 * k;
+      const float4 u0 = *reinterpret_cast<const float4*>(src + 4 * kb);
+      const float4 u1 = *reinterpret_cast<const float4*>(src + 4 * (kb ^ 1));
+      if (raw) {
+        // split-K partial: raw fp32 rows -> partial[t][row][64]
+        float* dst = p.partial + (static_cast<size_t>(t) * kTileM + row) * 64 + 8 * k;
+        *reinterpret_cast<float4*>(dst) = u0;
+        *reinterpret_cast<float4*>(dst + 4) = u1;
+        continue;
+      }
+      const float y[8] = {u0.x, u0.y, u0.z, u0.w, u1.x, u1.y, u1.z, u1.w};
+      uint32_t hi[4], lo[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint2 o = finish_pair<NL>(p, y[2 * j], y[2 * j + 1], rw[i], j);
+        hi[j] = o.x; lo[j] = o.y;
+      }
+      *reinterpret_cast<uint4*>(out[i]) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+      if (NL == 2) *reinterpret_cast<uint4*>(out[i] + p.out_limb_stride) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
     }
   }
 }
@@ -526,6 +622,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_umma_kernel(const __grid_con
 // A and B move through separate mbarrier rings: an A patch is consumed by n_taps B tiles.
 // The consumers ping-pong: warpgroup 1 owns the CTA's even local tiles and warpgroup 2 the odd ones, all 128 rows of
 // each (two m64nBN accumulators), so one warpgroup runs its epilogue while the other issues the next tile's MMAs.
+// BN = 64 (not the tail) transposes the tile instead: the weight tile is the wgmma A operand (64 rows, SBO 1024) and the
+// patch at the tap's row the B operand with N = 128 (the 16 core-matrix groups are the 16 image rows, SBO = PW * 128 B
+// apart), one m64n128k16 per limb product where two m64n64k16 read 4 KB of shared memory per 32 tensor cycles.
 // ====================================================================================================
 constexpr int kPatchSlot = 23 * 1024;           // >= 10*18*128 = 23040 bytes
 constexpr int kPatchStride = 23 * 1024;         // distance between patch buffers (1024-byte aligned)
@@ -538,7 +637,9 @@ static_assert(128 * kProducerRegs + 256 * kConsumerRegs <= 65536, "register file
 
 template <int BN, int NL, bool TAIL>
 struct PatchCfg {
-  using Aux = AuxCfg<TAIL>;
+  using Aux = AuxCfg<BN, TAIL>;
+  // BN = 64 (not the tail) computes the transposed tile D^T[64 channels x 128 pixels] with one m64n128 accumulator
+  static constexpr bool kCols = BN == 64 && !TAIL;
   static constexpr int kBTile = BN * 128;
   // taps per B stage: each stage costs one barrier round trip, so a stage must carry enough tensor work: 2 taps for
   // N=128 bf16, 2-3 for N=64, all 9 for the tail.
@@ -573,7 +674,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
   uint64_t* bfull_bar = aempty_bar + Cfg::kAStages;         // [kBStages]
   uint64_t* bempty_bar = bfull_bar + Cfg::kBStages;         // [kBStages]
   uint64_t* turn_bar = bempty_bar + Cfg::kBStages;          // [2]: consumer warpgroup w has issued every MMA of a tile
-  float* tail_stg = reinterpret_cast<float*>(aux + kBarBytes);
+  float* stg_base = reinterpret_cast<float*>(aux + kBarBytes);   // epilogue staging, half per consumer warpgroup
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);   // provably warp-uniform
   const int lane = threadIdx.x & 31;
@@ -678,8 +779,9 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
     ptx::setmaxnreg_inc<kConsumerRegs>();
     // ===================================================================== consumers (warpgroups 1, 2)
     // Ping-pong: warpgroup w owns the local tiles lt with lt % 2 == w, all 128 rows (acc[0]: rows 0-63, acc[1]: rows
-    // 64-127, read 8 image rows further down the patch).  Every accumulator element sees the same operands in the same
-    // K order as one m64 half of a tile split across both warpgroups would.  A ring stage is consumed by the warpgroup
+    // 64-127, read 8 image rows further down the patch; BN = 64: acc[0] = the transposed tile, channels x 128 rows).
+    // Every accumulator element sees the same operands in the same K order as one m64 half of a tile split across both
+    // warpgroups would.  A ring stage is consumed by the warpgroup
     // that owns its tile; the other one moves its cursors past the tile's stages.
     // MMA issue alternates by tile: tile lt > 0 starts once the other warpgroup has issued every MMA of tile lt-1
     // (turn_bar), so the tensor pipe finishes one tile before it starts the next and the owner's epilogue runs under the
@@ -693,7 +795,7 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
     uint32_t pha = 0, phb = 0;
     const uint32_t sbo = static_cast<uint32_t>(p.patch_w) * 128u;
     const uint32_t row_off = static_cast<uint32_t>(8 * p.patch_w) * 128u;   // tile rows 64..127: 8 image rows down
-    float* stg = tail_stg + wg * kTileM * kTailStride;                       // this warpgroup's tail staging (128 rows)
+    float* stg = stg_base + wg * (Cfg::Aux::kStgBytes / 8);                 // this warpgroup's staging
     int lt = 0;
     for (int t = t0; t < p.total_tiles; t += tstep, ++lt) {
       const TileCoord tc = decode_tile(p, t);
@@ -711,11 +813,12 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
       }
       if (lt > 0) ptx::mbar_wait(&turn_bar[wg ^ 1], static_cast<uint32_t>((lt - 1) >> 1) & 1u);
       if (wg_leader) trace_tile(p, lt, 0);
-      float acc[2][BN / 2];
+      constexpr int kHalves = Cfg::kCols ? 1 : 2, kAccN = Cfg::kCols ? kTileM : BN;
+      float acc[kHalves][kAccN / 2];
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
+      for (int h = 0; h < kHalves; ++h)
 #pragma unroll
-        for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.0f;
+        for (int i = 0; i < kAccN / 2; ++i) acc[h][i] = 0.0f;
       // the stage consumed one step earlier is released once the MMAs that read it have retired (wgmma.wait_group 1)
       int prev_b = -1, prev_a = -1;
       for (int ci = ci0; ci < ci1; ++ci) {
@@ -738,14 +841,26 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
 #pragma unroll
               for (int k = 0; k < kChunk / 16; ++k) {
                 const uint32_t accum = (ci > ci0 || tap > 0 || k > 0) ? 1u : 0u;
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                  const uint64_t a_hi = ptx::gmma_desc_sw128(a_hi_addr + h * row_off, sbo);
-                  ptx::wgmma_m64k16<BN, NL == 2>(acc[h], a_hi + 2 * k, b_hi + 2 * k, accum);
+                if constexpr (Cfg::kCols) {
+                  // weights x pixels: the weight tile is the A operand, the patch the B operand with N = 128 (its 16
+                  // 8-row core-matrix groups are the tile's 16 image rows, one SBO apart); same products, same order
+                  const uint64_t x_hi = ptx::gmma_desc_sw128(a_hi_addr, sbo);
+                  ptx::wgmma_m64k16<kTileM, NL == 2>(acc[0], b_hi + 2 * k, x_hi + 2 * k, accum);
                   if constexpr (NL == 2) {
-                    const uint64_t a_lo = ptx::gmma_desc_sw128(a_hi_addr + h * row_off + kPatchStride, sbo);
-                    ptx::wgmma_m64k16<BN, true>(acc[h], a_hi + 2 * k, b_lo + 2 * k, 1u);
-                    ptx::wgmma_m64k16<BN, true>(acc[h], a_lo + 2 * k, b_hi + 2 * k, 1u);
+                    const uint64_t x_lo = ptx::gmma_desc_sw128(a_hi_addr + kPatchStride, sbo);
+                    ptx::wgmma_m64k16<kTileM, true>(acc[0], b_lo + 2 * k, x_hi + 2 * k, 1u);
+                    ptx::wgmma_m64k16<kTileM, true>(acc[0], b_hi + 2 * k, x_lo + 2 * k, 1u);
+                  }
+                } else {
+#pragma unroll
+                  for (int h = 0; h < kHalves; ++h) {
+                    const uint64_t a_hi = ptx::gmma_desc_sw128(a_hi_addr + h * row_off, sbo);
+                    ptx::wgmma_m64k16<BN, NL == 2>(acc[h], a_hi + 2 * k, b_hi + 2 * k, accum);
+                    if constexpr (NL == 2) {
+                      const uint64_t a_lo = ptx::gmma_desc_sw128(a_hi_addr + h * row_off + kPatchStride, sbo);
+                      ptx::wgmma_m64k16<BN, true>(acc[h], a_hi + 2 * k, b_lo + 2 * k, 1u);
+                      ptx::wgmma_m64k16<BN, true>(acc[h], a_lo + 2 * k, b_hi + 2 * k, 1u);
+                    }
                   }
                 }
               }
@@ -770,9 +885,13 @@ __global__ void __launch_bounds__(kThreads, 1) conv_patch_kernel(const __grid_co
         if (prev_a >= 0) ptx::mbar_arrive(&aempty_bar[prev_a]);
       }
       if (wg_leader) trace_tile(p, lt, 2);
+      if constexpr (Cfg::kCols) {
+        epilogue_cols<NL>(p, acc[0], tc, t, stg, 1 + wg);
+      } else {
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
-        epilogue_regs<BN, NL, TAIL>(p, acc[h], tc, t, 64 * h, stg + 64 * h * kTailStride, 1 + wg);
+        for (int h = 0; h < kHalves; ++h)
+          epilogue_regs<BN, NL, TAIL>(p, acc[h], tc, t, 64 * h, stg + 64 * h * kTailStride, 1 + wg);
+      }
       if (wg_leader) trace_tile(p, lt, 3);
     }
   }
