@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h and include/lspm.h.  Plain pointers and sizes only."""
+"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h and include/lspa.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
 import ctypes as C
@@ -26,6 +26,9 @@ SYMBOLS_H = ["lsph_create", "lsph_load_weights", "lsph_generate", "lsph_receptiv
 # include/lspm.h (APC manifold projection: KNN + LLE)
 SYMBOLS_M = ["lspm_create", "lspm_load_database", "lspm_workspace_bytes", "lspm_knn", "lspm_project", "lspm_destroy",
              "lspm_last_error"]
+
+# include/lspa.h (log-mel front end)
+SYMBOLS_A = ["lspa_create", "lspa_load_mel_basis", "lspa_logmel", "lspa_destroy", "lspa_last_error"]
 
 
 class LsphConfig(C.Structure):
@@ -141,6 +144,15 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     for name in SYMBOLS_M:
         if name != "lspm_last_error":
             getattr(lib, name).restype = C.c_int
+    lib.lspa_last_error.restype = C.c_char_p
+    lib.lspa_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
+    lib.lspa_load_mel_basis.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
+    lib.lspa_logmel.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_int, C.c_void_p,
+                                C.c_void_p]
+    lib.lspa_destroy.argtypes = [C.c_void_p]
+    for name in SYMBOLS_A:
+        if name != "lspa_last_error":
+            getattr(lib, name).restype = C.c_int
     _LIB = lib
     return lib
 
@@ -158,3 +170,8 @@ def check_h(code: int) -> None:
 def check_m(code: int) -> None:
     if code != 0:
         raise LspgError(code, (load().lspm_last_error() or b"").decode("utf-8", "replace"))
+
+
+def check_a(code: int) -> None:
+    if code != 0:
+        raise LspgError(code, (load().lspa_last_error() or b"").decode("utf-8", "replace"))
