@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h and include/lspa.h.  Plain pointers and sizes only."""
+"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h and include/lspl.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
 import ctypes as C
@@ -30,10 +30,26 @@ SYMBOLS_M = ["lspm_create", "lspm_load_database", "lspm_workspace_bytes", "lspm_
 # include/lspa.h (log-mel front end)
 SYMBOLS_A = ["lspa_create", "lspa_load_mel_basis", "lspa_logmel", "lspa_destroy", "lspa_last_error"]
 
+# include/lspl.h (landmark post-processing, demo.py stage 5)
+SYMBOLS_L = ["lspl_create", "lspl_load_identity", "lspl_workspace_bytes", "lspl_run", "lspl_destroy", "lspl_last_error"]
+
 
 class LsphConfig(C.Structure):
     _fields_ = [(k, C.c_int) for k in ("apc_hidden", "frame_future", "layers", "blocks", "residual_ch", "dilation_ch", "skip_ch",
                                        "kernel_size", "use_bias", "cond_ch", "input_ch", "ncenter", "ndim", "loss_gmm")]
+
+
+class LsplIdentity(C.Structure):
+    _fields_ = [("mean_pts3d", C.c_void_p), ("std_mean_pts3d", C.c_void_p), ("candidate_eye_brow", C.c_void_p),
+                ("n_candidates", C.c_int), ("mean_translation", C.c_double * 3), ("ref_trans", C.c_double * 3),
+                ("shoulder3D", C.c_void_p), ("camera_intrinsic", C.c_double * 9), ("relative_rotation", C.c_double * 9),
+                ("relative_translation", C.c_double * 3), ("scale", C.c_double)]
+
+
+class LsplParams(C.Structure):
+    _fields_ = [("feat_sigma", C.c_double), ("rot_sigma", C.c_double), ("trans_sigma", C.c_double),
+                ("amp", (C.c_double * 3) * 18), ("rot_amp", C.c_double), ("trans_amp", C.c_double),
+                ("shoulder_amp", C.c_double), ("use_pad", C.c_int), ("pad", C.c_int * 4)]
 
 
 class LspgTensor(C.Structure):
@@ -153,6 +169,16 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     for name in SYMBOLS_A:
         if name != "lspa_last_error":
             getattr(lib, name).restype = C.c_int
+    lib.lspl_last_error.restype = C.c_char_p
+    lib.lspl_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
+    lib.lspl_load_identity.argtypes = [C.c_void_p, C.POINTER(LsplIdentity)]
+    lib.lspl_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
+    lib.lspl_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsplParams), C.c_void_p,
+                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
+    lib.lspl_destroy.argtypes = [C.c_void_p]
+    for name in SYMBOLS_L:
+        if name != "lspl_last_error":
+            getattr(lib, name).restype = C.c_int
     _LIB = lib
     return lib
 
@@ -175,3 +201,8 @@ def check_m(code: int) -> None:
 def check_a(code: int) -> None:
     if code != 0:
         raise LspgError(code, (load().lspa_last_error() or b"").decode("utf-8", "replace"))
+
+
+def check_l(code: int) -> None:
+    if code != 0:
+        raise LspgError(code, (load().lspl_last_error() or b"").decode("utf-8", "replace"))

@@ -81,14 +81,22 @@ def mux_audio(video_path: str, audio_path: str, output_path: str) -> bool:
     return True
 
 
-def render_to_video(net, landmarks: np.ndarray, shoulders: Optional[np.ndarray], cand_device: torch.Tensor, output_path: str,
+def _tracks(x, dev):
+    """A CUDA tensor stays on the device (fp32, contiguous); numpy goes to pinned host memory for one upload."""
+    if isinstance(x, torch.Tensor) and x.is_cuda:
+        return x.to(device=dev, dtype=torch.float32).contiguous()
+    return torch.from_numpy(np.ascontiguousarray(x, dtype=np.float32)).pin_memory()
+
+
+def render_to_video(net, landmarks, shoulders, cand_device: torch.Tensor, output_path: str,
                     size: tuple = (512, 512), fps: float = 60.0, batch: int = 32, fourcc: str = "DIVX",
                     audio_path: Optional[str] = None, feature_maps_path: Optional[str] = None,
                     precision: Optional[str] = None) -> dict:
     """Render a clip from its landmark tracks straight into a video file.
 
     ``landmarks`` [N,73,2] and ``shoulders`` [N,18,2] (or None) are the per-frame tracks demo.py:237-258 computes
-    (``pred_landmarks`` / ``pred_shoulders``); ``cand_device`` is ``img_candidates`` (demo.py:95).  ``size`` = (W, H) =
+    (``pred_landmarks`` / ``pred_shoulders``), as numpy or as CUDA tensors (``LandmarkPostprocessor.run``'s output, used
+    without a host round trip); ``cand_device`` is ``img_candidates`` (demo.py:95).  ``size`` = (W, H) =
     ``(opt.loadSize, opt.loadSize)``.  ``feature_maps_path``: also write the rasterised input maps as a second video
     (demo.py:282-283, ``save_feature_maps``).  ``audio_path``: mux it like demo.py:43-44 when an ffmpeg binary exists.
     Returns ``{"frames", "seconds", "encode_seconds", "writer", "audio_muxed"}``.
@@ -96,8 +104,8 @@ def render_to_video(net, landmarks: np.ndarray, shoulders: Optional[np.ndarray],
     n = int(landmarks.shape[0])
     w, h = int(size[0]), int(size[1])
     dev = cand_device.device
-    lm_host = torch.from_numpy(np.ascontiguousarray(landmarks, dtype=np.float32)).pin_memory()
-    sh_host = None if shoulders is None else torch.from_numpy(np.ascontiguousarray(shoulders, dtype=np.float32)).pin_memory()
+    lm_tracks = _tracks(landmarks, dev)
+    sh_tracks = None if shoulders is None else _tracks(shoulders, dev)
     frames_host = torch.empty((n, h, w, 3), dtype=torch.uint8).pin_memory()
     frames_np = frames_host.numpy()
     want_mux = audio_path is not None and shutil.which("ffmpeg") is not None
@@ -109,7 +117,7 @@ def render_to_video(net, landmarks: np.ndarray, shoulders: Optional[np.ndarray],
     wt = _WriterThread(_open_writer(video_path, fps, (w, h), fourcc))
     clip = ClipRenderer(net, batch=batch, device=dev, precision=precision, uint8=True)
     try:
-        clip.render_clip_from_landmarks(lm_host, sh_host, cand_device, frames_host, (w, h),
+        clip.render_clip_from_landmarks(lm_tracks, sh_tracks, cand_device, frames_host, (w, h),
                                         on_batch=lambda off, ln: wt.put(frames_np[off:off + ln]))
     finally:
         wt.close()
@@ -118,8 +126,8 @@ def render_to_video(net, landmarks: np.ndarray, shoulders: Optional[np.ndarray],
     if feature_maps_path is not None:
         fw = _WriterThread(_open_writer(feature_maps_path, fps, (w, h), fourcc))
         try:
-            lm_dev = lm_host.to(dev)
-            sh_dev = None if sh_host is None else sh_host.to(dev)
+            lm_dev = lm_tracks.to(dev)
+            sh_dev = None if sh_tracks is None else sh_tracks.to(dev)
             for off in range(0, n, batch):
                 fm = net.draw_feature_maps(lm_dev[off:off + batch], None if sh_dev is None else sh_dev[off:off + batch], (w, h))
                 gray = (fm[:, 0] * 255.0).to(torch.uint8).cpu().numpy()                   # demo.py:270: np.uint8(map * 255)
