@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h and include/lspl.h.  Plain pointers and sizes only."""
+"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h and include/lspr.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
 import ctypes as C
@@ -33,10 +33,19 @@ SYMBOLS_A = ["lspa_create", "lspa_load_mel_basis", "lspa_logmel", "lspa_destroy"
 # include/lspl.h (landmark post-processing, demo.py stage 5)
 SYMBOLS_L = ["lspl_create", "lspl_load_identity", "lspl_workspace_bytes", "lspl_run", "lspl_destroy", "lspl_last_error"]
 
+# include/lspr.h (APC encoder GRU and Audio2Mouth LSTM, demo.py stages 1 and 3)
+SYMBOLS_R = ["lspr_create", "lspr_load_weights", "lspr_workspace_bytes", "lspr_forward", "lspr_debug_packed", "lspr_destroy",
+             "lspr_last_error"]
+LSPR_KIND = {"apc": 0, "mouth": 1}
+
 
 class LsphConfig(C.Structure):
     _fields_ = [(k, C.c_int) for k in ("apc_hidden", "frame_future", "layers", "blocks", "residual_ch", "dilation_ch", "skip_ch",
                                        "kernel_size", "use_bias", "cond_ch", "input_ch", "ncenter", "ndim", "loss_gmm")]
+
+
+class LsprConfig(C.Structure):
+    _fields_ = [(k, C.c_int) for k in ("kind", "input_dim", "hidden", "num_layers", "residual", "frame_future", "out_dim")]
 
 
 class LsplIdentity(C.Structure):
@@ -179,6 +188,16 @@ def load(build_if_missing: bool = True) -> C.CDLL:
     for name in SYMBOLS_L:
         if name != "lspl_last_error":
             getattr(lib, name).restype = C.c_int
+    lib.lspr_last_error.restype = C.c_char_p
+    lib.lspr_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(LsprConfig), C.c_int]
+    lib.lspr_load_weights.argtypes = [C.c_void_p, C.POINTER(LspgTensor), C.c_int]
+    lib.lspr_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_size_t)]
+    lib.lspr_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
+    lib.lspr_debug_packed.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int64)]
+    lib.lspr_destroy.argtypes = [C.c_void_p]
+    for name in SYMBOLS_R:
+        if name != "lspr_last_error":
+            getattr(lib, name).restype = C.c_int
     _LIB = lib
     return lib
 
@@ -206,3 +225,8 @@ def check_a(code: int) -> None:
 def check_l(code: int) -> None:
     if code != 0:
         raise LspgError(code, (load().lspl_last_error() or b"").decode("utf-8", "replace"))
+
+
+def check_r(code: int) -> None:
+    if code != 0:
+        raise LspgError(code, (load().lspr_last_error() or b"").decode("utf-8", "replace"))

@@ -34,6 +34,7 @@
 #include <vector>
 
 #include "../../include/lsph.h"
+#include "gemm_nt.cuh"
 
 namespace cg = cooperative_groups;
 
@@ -63,52 +64,7 @@ constexpr int kMaxLayers = 16;      // layers x blocks (14 for the shipped optio
 constexpr int kMaxIn = 32;
 constexpr int kMaxOut = 128;
 
-// ------------------------------------------------------------------------------------------------
-// GEMM for the hoisted audio path:  C[M,N] = epilogue( A[M,K] * W[N,K]^T ),  epilogue v -> v*scale[n] + shift[n], LeakyReLU
-// 64x64 tile, K step 16, 256 threads x (4x4) outputs.  N % 64 == 0 and K % 16 == 0 (512 / 1024 / 3584 here); M ragged.
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) gemm_nt_kernel(const float* __restrict__ A, const float* __restrict__ W,
-                                                      const float* __restrict__ scale, const float* __restrict__ shift,
-                                                      float* __restrict__ C, int M, int N, int K, int leaky) {
-  __shared__ float As[16][64 + 4];
-  __shared__ float Ws[16][64 + 4];
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  const int m0 = blockIdx.y * 64, n0 = blockIdx.x * 64;
-  float acc[4][4] = {};
-  const int lr = threadIdx.x >> 2;            // 0..63: tile row loaded by this thread
-  const int lk = (threadIdx.x & 3) * 4;       // 0,4,8,12: first of its 4 k values
-  for (int k0 = 0; k0 < K; k0 += 16) {
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (m0 + lr < M) a = *reinterpret_cast<const float4*>(A + static_cast<size_t>(m0 + lr) * K + k0 + lk);
-    const float4 w = *reinterpret_cast<const float4*>(W + static_cast<size_t>(n0 + lr) * K + k0 + lk);
-    As[lk + 0][lr] = a.x; As[lk + 1][lr] = a.y; As[lk + 2][lr] = a.z; As[lk + 3][lr] = a.w;
-    Ws[lk + 0][lr] = w.x; Ws[lk + 1][lr] = w.y; Ws[lk + 2][lr] = w.z; Ws[lk + 3][lr] = w.w;
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < 16; ++k) {
-      float av[4], wv[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) { av[i] = As[k][ty * 4 + i]; wv[i] = Ws[k][tx * 4 + i]; }
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], wv[j], acc[i][j]);
-    }
-    __syncthreads();
-  }
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int m = m0 + ty * 4 + i;
-    if (m >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int n = n0 + tx * 4 + j;
-      float v = fmaf(acc[i][j], scale[n], shift[n]);
-      if (leaky) v = v > 0.f ? v : 0.2f * v;
-      C[static_cast<size_t>(m) * N + n] = v;
-    }
-  }
-}
+// The hoisted audio path (audio_downsample and the conditioning projections) runs on gemm_nt_kernel (csrc/gemm_nt.cuh).
 
 // ------------------------------------------------------------------------------------------------
 // The autoregressive kernel
@@ -632,9 +588,9 @@ int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const fl
   // ---- hoisted audio path: downsample every row, project it for every block
   const dim3 blk(256);
   const int mt = (n_audio + 63) / 64;
-  gemm_nt_kernel<<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, h->d_ds1, n_audio, H, 2 * H, 1);
-  gemm_nt_kernel<<<dim3(H / 64, mt), blk, 0, st>>>(h->d_ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, h->d_ds2, n_audio, H, H, 0);
-  gemm_nt_kernel<<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(h->d_ds2, h->d_w_cond, h->d_one, h->d_b_cond, h->d_cond, n_audio, L * 2 * kR, H, 0);
+  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, h->d_ds1, n_audio, H, 2 * H, 1, 0);
+  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(h->d_ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, h->d_ds2, n_audio, H, H, 0, 0);
+  gemm_nt_kernel<><<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(h->d_ds2, h->d_w_cond, h->d_one, h->d_b_cond, h->d_cond, n_audio, L * 2 * kR, H, 0, 0);
   HCUDA_TRY(cudaGetLastError());
   LoopParams p;
   memset(&p, 0, sizeof(p));
