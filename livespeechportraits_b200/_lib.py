@@ -1,41 +1,18 @@
 """ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h and include/lspr.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
+import functools
 import os
-from typing import Optional
+from typing import List, Optional, Tuple
+
+import torch
 
 from . import build as _build
 
 LSPG_VARIANT = {"normal": 0, "large": 1}
 LSPG_MODE = {"fast": 0, "parity": 1}
-
-SYMBOLS = [
-    "lspg_create", "lspg_load_weights", "lspg_workspace_bytes", "lspg_forward", "lspg_forward_image", "lspg_draw_feature_maps", "lspg_destroy",
-    "lspg_last_error",
-    "lspg_num_layers", "lspg_layer_info_get", "lspg_layer_packed", "lspg_layer_affine", "lspg_num_tensors",
-    "lspg_tensor_shape", "lspg_debug_read_tensor", "lspg_launches_per_forward", "lspg_flops_per_frame",
-    "lspg_profile_enable", "lspg_profile_read", "lspg_debug_read_trace", "lspg_debug_fast_div", "lspg_debug_layer_geo",
-    "lspg_graph_stats", "lspg_release_workspace",
-]
-
-# include/lsph.h (Audio2Headpose generation loop)
-SYMBOLS_H = ["lsph_create", "lsph_load_weights", "lsph_generate", "lsph_receptive_field", "lsph_debug_packed", "lsph_destroy",
-             "lsph_last_error"]
-
-# include/lspm.h (APC manifold projection: KNN + LLE)
-SYMBOLS_M = ["lspm_create", "lspm_load_database", "lspm_workspace_bytes", "lspm_knn", "lspm_project", "lspm_destroy",
-             "lspm_last_error"]
-
-# include/lspa.h (log-mel front end)
-SYMBOLS_A = ["lspa_create", "lspa_load_mel_basis", "lspa_logmel", "lspa_destroy", "lspa_last_error"]
-
-# include/lspl.h (landmark post-processing, demo.py stage 5)
-SYMBOLS_L = ["lspl_create", "lspl_load_identity", "lspl_workspace_bytes", "lspl_run", "lspl_destroy", "lspl_last_error"]
-
-# include/lspr.h (APC encoder GRU and Audio2Mouth LSTM, demo.py stages 1 and 3)
-SYMBOLS_R = ["lspr_create", "lspr_load_weights", "lspr_workspace_bytes", "lspr_forward", "lspr_debug_packed", "lspr_destroy",
-             "lspr_last_error"]
 LSPR_KIND = {"apc": 0, "mouth": 1}
 
 
@@ -82,6 +59,89 @@ class LspgLayerGeo(C.Structure):
                 ("w_box_taps", C.c_int * 2)]
 
 
+
+
+_p, _i, _i64, _sz = C.c_void_p, C.c_int, C.c_int64, C.c_size_t      # handles, device pointers and streams are _p
+_out_handle, _pi, _pi64, _psz = C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int64), C.POINTER(C.c_size_t)
+_tensors = C.POINTER(LspgTensor)
+_forward = [_p, _p, _i64, _p, _i64, _p, _i, _i, _i, _p, _sz, _i, _p]
+
+# Every C-ABI symbol and its argument types.  restype is c_char_p for *_last_error and c_int (0 or LSPG_E*) otherwise.
+ARGTYPES = {
+    # include/lspg.h (Feature2Face generator and feature-map rasteriser)
+    "lspg_create": [_out_handle, _i, _i, _i, _i, _i, _i],
+    "lspg_load_weights": [_p, _tensors, _i],
+    "lspg_workspace_bytes": [_p, _i, _i, _i, _i, _psz],
+    "lspg_forward": _forward,
+    "lspg_forward_image": _forward,
+    "lspg_draw_feature_maps": [_p, _p, _p, _i, _p, _i, _i, _i, _p],
+    "lspg_destroy": [_p],
+    "lspg_last_error": [],
+    "lspg_num_layers": [_p, _pi],
+    "lspg_layer_info_get": [_p, _i, C.POINTER(LspgLayerInfo)],
+    "lspg_layer_packed": [_p, _i, _i, _p, _i64],
+    "lspg_layer_affine": [_p, _i, _p, _p, _i64],
+    "lspg_num_tensors": [_p, _pi],
+    "lspg_tensor_shape": [_p, _i, _i, _i, _pi, _pi, _pi],
+    "lspg_debug_read_tensor": [_p, _i, _i, _p, _i64],
+    "lspg_launches_per_forward": [_p, _pi],
+    "lspg_flops_per_frame": [_p, _i, _i, C.POINTER(C.c_double)],
+    "lspg_profile_enable": [_p, _i],
+    "lspg_profile_read": [_p, _p, _i, _pi],
+    "lspg_debug_read_trace": [_p, _p, _i64],
+    "lspg_debug_fast_div": [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)],
+    "lspg_debug_layer_geo": [_p, _i, _i, _i, _i, C.POINTER(LspgLayerGeo)],
+    "lspg_graph_stats": [_p, _pi64, _pi64, _pi64],
+    "lspg_release_workspace": [_p, _p],
+    # include/lsph.h (Audio2Headpose generation loop)
+    "lsph_create": [_out_handle, C.POINTER(LsphConfig), _i],
+    "lsph_load_weights": [_p, _tensors, _i],
+    "lsph_generate": [_p, _p, _i, _p, _p, _p, C.c_float, _p, _p, _i, _p],
+    "lsph_receptive_field": [_p, _pi],
+    "lsph_debug_packed": [_p, _i, _p, _i64],
+    "lsph_destroy": [_p],
+    "lsph_last_error": [],
+    # include/lspm.h (APC manifold projection: KNN + LLE)
+    "lspm_create": [_out_handle, _i, _i],
+    "lspm_load_database": [_p, _p, _i64],
+    "lspm_workspace_bytes": [_p, _i, _i, _psz],
+    "lspm_knn": [_p, _p, _i, _i, _p, _p, _p, _sz, _p],
+    "lspm_project": [_p, _p, _i, _p, _i, C.c_float, _p, _p, _p, _p, _p],
+    "lspm_destroy": [_p],
+    "lspm_last_error": [],
+    # include/lspa.h (log-mel front end)
+    "lspa_create": [_out_handle, _i],
+    "lspa_load_mel_basis": [_p, _p, _i, _i],
+    "lspa_logmel": [_p, _p, _i64, _i, _i, C.c_double, _i, _p, _p],
+    "lspa_destroy": [_p],
+    "lspa_last_error": [],
+    # include/lspl.h (landmark post-processing, demo.py stage 5)
+    "lspl_create": [_out_handle, _i],
+    "lspl_load_identity": [_p, C.POINTER(LsplIdentity)],
+    "lspl_workspace_bytes": [_p, _i, _i, _psz],
+    "lspl_run": [_p, _p, _i, _p, _i, _i, C.POINTER(LsplParams), _p, _p, _p, _p, _p, _sz, _p],
+    "lspl_destroy": [_p],
+    "lspl_last_error": [],
+    # include/lspr.h (APC encoder GRU and Audio2Mouth LSTM, demo.py stages 1 and 3)
+    "lspr_create": [_out_handle, C.POINTER(LsprConfig), _i],
+    "lspr_load_weights": [_p, _tensors, _i],
+    "lspr_workspace_bytes": [_p, _i, _psz],
+    "lspr_forward": [_p, _p, _i, _p, _p, _sz, _i, _p],
+    "lspr_debug_packed": [_p, _i, _p, _pi64],
+    "lspr_destroy": [_p],
+    "lspr_last_error": [],
+}
+
+
+def symbols(prefix: Optional[str] = None) -> List[str]:
+    """The bound symbols of one module (``"lspm"``, ...), or of all six."""
+    return [name for name in ARGTYPES if prefix is None or name.startswith(prefix + "_")]
+
+
+# Per-module names that callers outside the package (tests, scripts) use: views of the table and of check().
+SYMBOLS, SYMBOLS_H, SYMBOLS_M, SYMBOLS_A, SYMBOLS_L, SYMBOLS_R = (symbols(p) for p in ("lspg", "lsph", "lspm", "lspa", "lspl", "lspr"))
+
+
 class LspgError(RuntimeError):
     def __init__(self, code: int, message: str):
         super().__init__(f"lspg error {code}: {message}")
@@ -116,117 +176,101 @@ def load(build_if_missing: bool = True) -> C.CDLL:
             warnings.warn(f"liblspg.so is older than its sources and could not be rebuilt ({exc}); using the existing binary",
                           RuntimeWarning)
     lib = C.CDLL(path)
-    lib.lspg_last_error.restype = C.c_char_p
-    lib.lspg_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
-    lib.lspg_load_weights.argtypes = [C.c_void_p, C.POINTER(LspgTensor), C.c_int]
-    lib.lspg_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
-    lib.lspg_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int,
-                                 C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
-    lib.lspg_forward_image.argtypes = lib.lspg_forward.argtypes
-    lib.lspg_debug_layer_geo.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(LspgLayerGeo)]
-    lib.lspg_debug_fast_div.argtypes = [C.c_uint32, C.c_uint32, C.POINTER(C.c_uint32)]
-    lib.lspg_draw_feature_maps.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int,
-                                           C.c_void_p]
-    lib.lspg_destroy.argtypes = [C.c_void_p]
-    lib.lspg_release_workspace.argtypes = [C.c_void_p, C.c_void_p]
-    lib.lspg_graph_stats.argtypes = [C.c_void_p, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
-    lib.lspg_num_layers.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
-    lib.lspg_layer_info_get.argtypes = [C.c_void_p, C.c_int, C.POINTER(LspgLayerInfo)]
-    lib.lspg_layer_packed.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64]
-    lib.lspg_layer_affine.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int64]
-    lib.lspg_num_tensors.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
-    lib.lspg_tensor_shape.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
-                                      C.POINTER(C.c_int)]
-    lib.lspg_debug_read_tensor.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64]
-    lib.lspg_launches_per_forward.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
-    lib.lspg_debug_read_trace.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-    lib.lspg_profile_enable.argtypes = [C.c_void_p, C.c_int]
-    lib.lspg_profile_read.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int)]
-    lib.lspg_flops_per_frame.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_double)]
-    for name in SYMBOLS:
-        if name != "lspg_last_error":
-            getattr(lib, name).restype = C.c_int
-    lib.lsph_last_error.restype = C.c_char_p
-    lib.lsph_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(LsphConfig), C.c_int]
-    lib.lsph_load_weights.argtypes = [C.c_void_p, C.POINTER(LspgTensor), C.c_int]
-    lib.lsph_generate.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
-                                  C.c_void_p, C.c_int, C.c_void_p]
-    lib.lsph_receptive_field.argtypes = [C.c_void_p, C.POINTER(C.c_int)]
-    lib.lsph_destroy.argtypes = [C.c_void_p]
-    lib.lsph_debug_packed.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int64]
-    for name in SYMBOLS_H:
-        if name != "lsph_last_error":
-            getattr(lib, name).restype = C.c_int
-    lib.lspm_last_error.restype = C.c_char_p
-    lib.lspm_create.argtypes = [C.POINTER(C.c_void_p), C.c_int, C.c_int]
-    lib.lspm_load_database.argtypes = [C.c_void_p, C.c_void_p, C.c_int64]
-    lib.lspm_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
-    lib.lspm_knn.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
-                             C.c_void_p]
-    lib.lspm_project.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_float, C.c_void_p, C.c_void_p,
-                                 C.c_void_p, C.c_void_p, C.c_void_p]
-    lib.lspm_destroy.argtypes = [C.c_void_p]
-    for name in SYMBOLS_M:
-        if name != "lspm_last_error":
-            getattr(lib, name).restype = C.c_int
-    lib.lspa_last_error.restype = C.c_char_p
-    lib.lspa_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
-    lib.lspa_load_mel_basis.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int]
-    lib.lspa_logmel.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_int, C.c_void_p,
-                                C.c_void_p]
-    lib.lspa_destroy.argtypes = [C.c_void_p]
-    for name in SYMBOLS_A:
-        if name != "lspa_last_error":
-            getattr(lib, name).restype = C.c_int
-    lib.lspl_last_error.restype = C.c_char_p
-    lib.lspl_create.argtypes = [C.POINTER(C.c_void_p), C.c_int]
-    lib.lspl_load_identity.argtypes = [C.c_void_p, C.POINTER(LsplIdentity)]
-    lib.lspl_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_size_t)]
-    lib.lspl_run.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.POINTER(LsplParams), C.c_void_p,
-                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
-    lib.lspl_destroy.argtypes = [C.c_void_p]
-    for name in SYMBOLS_L:
-        if name != "lspl_last_error":
-            getattr(lib, name).restype = C.c_int
-    lib.lspr_last_error.restype = C.c_char_p
-    lib.lspr_create.argtypes = [C.POINTER(C.c_void_p), C.POINTER(LsprConfig), C.c_int]
-    lib.lspr_load_weights.argtypes = [C.c_void_p, C.POINTER(LspgTensor), C.c_int]
-    lib.lspr_workspace_bytes.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_size_t)]
-    lib.lspr_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p]
-    lib.lspr_debug_packed.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(C.c_int64)]
-    lib.lspr_destroy.argtypes = [C.c_void_p]
-    for name in SYMBOLS_R:
-        if name != "lspr_last_error":
-            getattr(lib, name).restype = C.c_int
+    for name, argtypes in ARGTYPES.items():
+        fn = getattr(lib, name)
+        fn.argtypes = argtypes
+        fn.restype = C.c_char_p if name.endswith("_last_error") else C.c_int
     _LIB = lib
     return lib
 
 
-def check(code: int) -> None:
+def check(code: int, prefix: str = "lspg") -> None:
+    """Raise ``LspgError`` with ``<prefix>_last_error()`` if a ``<prefix>_*`` call returned ``code != 0``."""
     if code != 0:
-        raise LspgError(code, (load().lspg_last_error() or b"").decode("utf-8", "replace"))
+        raise LspgError(code, (getattr(load(), prefix + "_last_error")() or b"").decode("utf-8", "replace"))
 
 
-def check_h(code: int) -> None:
-    if code != 0:
-        raise LspgError(code, (load().lsph_last_error() or b"").decode("utf-8", "replace"))
+check_h, check_m, check_a, check_l, check_r = (functools.partial(check, prefix=p) for p in ("lsph", "lspm", "lspa", "lspl", "lspr"))
 
 
-def check_m(code: int) -> None:
-    if code != 0:
-        raise LspgError(code, (load().lspm_last_error() or b"").decode("utf-8", "replace"))
+def cuda_device(device, what: str) -> torch.device:
+    """``device`` (None: the current CUDA device) as an indexed CUDA device; anything else is refused, as there is no CPU
+    path.  ``what`` names the caller in the refusal."""
+    if device is None:
+        device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
+    device = torch.device(device)
+    if device.type != "cuda":
+        raise RuntimeError(f"livespeechportraits_b200 has no CPU path: {what} needs an H100 (sm_90) device")
+    return device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
 
 
-def check_a(code: int) -> None:
-    if code != 0:
-        raise LspgError(code, (load().lspa_last_error() or b"").decode("utf-8", "replace"))
+def tensor_array(state_dict) -> Tuple[C.Array, list]:
+    """A state dict as the ``lspg_tensor`` array of the ``*_load_weights`` calls: fp32 contiguous CPU copies, without
+    BatchNorm's ``num_batches_tracked``.  The array points into ``keep``, which must outlive the call."""
+    keep = [(k.encode(), v.detach().to(device="cpu", dtype=torch.float32).contiguous())
+            for k, v in state_dict.items() if not k.endswith("num_batches_tracked")]
+    arr = (LspgTensor * len(keep))()
+    for e, (name, t) in zip(arr, keep):
+        e.name, e.data, e.numel = name, C.cast(t.data_ptr(), C.POINTER(C.c_float)), t.numel()
+    return arr, keep
 
 
-def check_l(code: int) -> None:
-    if code != 0:
-        raise LspgError(code, (load().lspl_last_error() or b"").decode("utf-8", "replace"))
+def cached(cache: dict, net, make, extra=()):
+    """The handle ``make(state_dict)`` built for the torch module ``net``, kept as the only entry of ``cache``.  It is
+    re-loaded (``load_state_dict``) when the module's tensors changed - version counters move on every in-place write
+    (load_state_dict, optimiser steps, init_weights), data pointers on re-allocation (``.to()``) - and rebuilt when
+    ``extra`` changed."""
+    sd = net.state_dict()
+    stamp = (tuple((v.data_ptr(), v._version) for v in sd.values()), tuple(extra))
+    hit = cache.get(id(net))
+    if hit is None or hit[1] != stamp:
+        if hit is not None and hit[1][1] == stamp[1]:
+            gen = hit[0]
+            gen.load_state_dict(sd)
+        else:
+            gen = make(sd)
+        cache.clear()
+        cache[id(net)] = (gen, stamp)
+    return cache[id(net)][0]
 
 
-def check_r(code: int) -> None:
-    if code != 0:
-        raise LspgError(code, (load().lspr_last_error() or b"").decode("utf-8", "replace"))
+class Handle:
+    """Owns one native handle of the C ABI ``<prefix>_*``: ``__init__`` resolves the device (-1: a host-only handle,
+    ``self.device`` None), ``_create`` calls ``<prefix>_create(&handle, *args, device)``, ``call`` makes checked calls
+    with the handle first, and ``__del__`` destroys it."""
+    prefix = ""
+    what = ""                      # names the subclass in the "no CPU path" refusal
+    _handle = None
+
+    def __init__(self, device):
+        self._lib = load()
+        self.device = None if device == -1 else cuda_device(device, self.what)
+
+    def _create(self, *args) -> None:
+        h = C.c_void_p()
+        check(getattr(self._lib, self.prefix + "_create")(C.byref(h), *args, -1 if self.device is None else self.device.index),
+              self.prefix)
+        self._handle = h
+
+    def call(self, name: str, *args) -> None:
+        check(getattr(self._lib, f"{self.prefix}_{name}")(self._handle, *args), self.prefix)
+
+    @contextlib.contextmanager
+    def stream(self):
+        """Enters the handle's device and yields its current stream (a ``cudaStream_t`` as int)."""
+        with torch.cuda.device(self.device):
+            yield torch.cuda.current_stream(self.device).cuda_stream
+
+    def workspace(self, *args) -> torch.Tensor:
+        """A device buffer of the ``<prefix>_workspace_bytes(handle, *args)`` bytes (at least one byte)."""
+        need = C.c_size_t()
+        self.call("workspace_bytes", *args, C.byref(need))
+        return torch.empty(max(need.value, 1), dtype=torch.uint8, device=self.device)
+
+    def __del__(self):
+        try:
+            if self._handle:
+                getattr(self._lib, self.prefix + "_destroy")(self._handle)
+                self._handle = None
+        except Exception:
+            pass

@@ -13,7 +13,6 @@ module attribute, so it then runs unchanged.  There is no CPU path.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional
 
 import numpy as np
@@ -92,19 +91,13 @@ def frame_len_of(sr, winlen) -> int:
 # ------------------------------------------------------------------------------------------------------------------
 # The device front end
 # ------------------------------------------------------------------------------------------------------------------
-class MelFrontEnd:
+class MelFrontEnd(_lib.Handle):
     """Owns the native handle and a device copy of the mel basis (fp32 [n_mels, 257], 1 <= n_mels <= 128; ``mel_basis()``
     by default).  The copy is taken at construction."""
+    prefix, what = "lspa", "the log-mel front end"
 
     def __init__(self, mel_basis=None, device: Optional[torch.device] = None):
-        self._lib = _lib.load()
-        self._handle = C.c_void_p()
-        if device is None:
-            device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: the log-mel front end needs an H100 (sm_90) device")
-        self.device = device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
+        super().__init__(device)
         basis = _default_basis() if mel_basis is None else mel_basis
         if isinstance(basis, torch.Tensor):
             basis = basis.detach().cpu().numpy()
@@ -112,8 +105,8 @@ class MelFrontEnd:
         if basis.ndim != 2 or basis.shape[1] != N_BINS or not 1 <= basis.shape[0] <= MAX_MELS:
             raise ValueError(f"mel_basis must be [n_mels <= {MAX_MELS}, {N_BINS}], got shape {basis.shape}")
         self.n_mels = basis.shape[0]
-        _lib.check_a(self._lib.lspa_create(C.byref(self._handle), self.device.index))
-        _lib.check_a(self._lib.lspa_load_mel_basis(self._handle, basis.ctypes.data, self.n_mels, N_BINS))
+        self._create()
+        self.call("load_mel_basis", basis.ctypes.data, self.n_mels, N_BINS)
 
     def logmel(self, audio, winlen: float = 1 / 60, winstep: float = 0.5 / 60, sr: int = 16000,
                normalize: bool = True) -> torch.Tensor:
@@ -128,19 +121,10 @@ class MelFrontEnd:
         a = a.to(device=self.device, dtype=torch.float32).contiguous()
         n = 2 * int(a.shape[0] / 16000 * 60)
         out = torch.empty((n, self.n_mels), dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            _lib.check_a(self._lib.lspa_logmel(self._handle, a.data_ptr() if a.numel() else None, a.shape[0], n, frame_len,
-                                               step, int(bool(normalize)), out.data_ptr() if n else None, stream))
+        with self.stream() as stream:
+            self.call("logmel", a.data_ptr() if a.numel() else None, a.shape[0], n, frame_len, step, int(bool(normalize)),
+                      out.data_ptr() if n else None, stream)
         return out
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.lspa_destroy(self._handle)
-                self._handle = C.c_void_p()
-        except Exception:
-            pass
 
 
 def compute_mel_one_sequence(audio, hop_length=int(16000 / 120), winlen=1 / 60, winstep=0.5 / 60, sr=16000, fps=60,

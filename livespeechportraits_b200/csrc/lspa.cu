@@ -22,31 +22,16 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
-#include <string>
 
 #include "../../include/lspa.h"
+#include "capi.cuh"
+
+using capi::DeviceGuard;
 
 namespace {
 
-thread_local std::string g_aerr;
-
-int afail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_aerr = buf;
-  return code;
-}
-
-#define ACUDA_TRY(expr)                                                                           \
-  do {                                                                                            \
-    cudaError_t _e = (expr);                                                                      \
-    if (_e != cudaSuccess) return afail(LSPG_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
+struct Lspa;
+constexpr auto fail = capi::fail<Lspa>;
 
 constexpr int kNfft = 512;
 constexpr int kBins = kNfft / 2 + 1;           // 257
@@ -165,14 +150,6 @@ __global__ void __launch_bounds__(kThreads) lspa_logmel_kernel(const float* __re
   for (int e = tid; e < nw * n_mels; e += kThreads) dst[e] = stage[e];
 }
 
-class DeviceGuard {
- public:
-  explicit DeviceGuard(int dev) { cudaGetDevice(&prev_); if (prev_ != dev) cudaSetDevice(dev); dev_ = dev; }
-  ~DeviceGuard() { if (prev_ != dev_) cudaSetDevice(prev_); }
- private:
-  int prev_ = 0, dev_ = 0;
-};
-
 }  // namespace
 
 struct lspa_ctx {
@@ -185,7 +162,7 @@ struct lspa_ctx {
 
 extern "C" {
 
-const char* lspa_last_error(void) { return g_aerr.c_str(); }
+const char* lspa_last_error(void) { return capi::last_error<Lspa>().c_str(); }
 
 int lspa_destroy(lspa_handle h) {
   if (!h) return LSPG_OK;
@@ -200,19 +177,10 @@ int lspa_destroy(lspa_handle h) {
 }
 
 int lspa_create(lspa_handle* out, int device) {
-  if (!out) return afail(LSPG_EINVAL, "null argument");
+  if (!out) return fail(LSPG_EINVAL, "null argument");
   *out = nullptr;
-  if (device < -1) return afail(LSPG_EINVAL, "device must be >= -1 (got %d)", device);
-  if (device >= 0) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) return afail(LSPG_ENODEV, "no CUDA device: %s", cudaGetErrorString(e));
-    if (device >= count) return afail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
-    cudaDeviceProp prop;
-    ACUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0)
-      return afail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device, prop.major, prop.minor);
-  }
+  cudaDeviceProp prop;
+  if (int rc = capi::check_device<Lspa>(device, &prop)) return rc;
   lspa_ctx* h = new lspa_ctx;
   h->device = device;
   if (device >= 0) {
@@ -231,7 +199,7 @@ int lspa_create(lspa_handle* out, int device) {
     if (e == cudaSuccess) e = cudaMemcpy(h->d_hann, hann, sizeof(hann), cudaMemcpyHostToDevice);
     if (e != cudaSuccess) {
       lspa_destroy(h);
-      return afail(LSPG_ECUDA, "lspa_create: %s", cudaGetErrorString(e));
+      return fail(LSPG_ECUDA, "lspa_create: %s", cudaGetErrorString(e));
     }
   }
   *out = h;
@@ -239,36 +207,36 @@ int lspa_create(lspa_handle* out, int device) {
 }
 
 int lspa_load_mel_basis(lspa_handle h, const float* host_basis, int n_mels, int n_bins) {
-  if (!h || !host_basis) return afail(LSPG_EINVAL, "null argument");
-  if (n_mels < 1 || n_mels > kMaxMels) return afail(LSPG_EINVAL, "n_mels must be in [1, %d] (got %d)", kMaxMels, n_mels);
-  if (n_bins != kBins) return afail(LSPG_EINVAL, "the basis must have %d columns (n_fft 512; got %d)", kBins, n_bins);
-  if (h->device < 0) return afail(LSPG_ENODEV, "host-only handle: lspa_load_mel_basis needs an sm_90 device (no CPU path exists)");
+  if (!h || !host_basis) return fail(LSPG_EINVAL, "null argument");
+  if (n_mels < 1 || n_mels > kMaxMels) return fail(LSPG_EINVAL, "n_mels must be in [1, %d] (got %d)", kMaxMels, n_mels);
+  if (n_bins != kBins) return fail(LSPG_EINVAL, "the basis must have %d columns (n_fft 512; got %d)", kBins, n_bins);
+  if (int rc = capi::require_device<Lspa>(h->device, "lspa_load_mel_basis")) return rc;
   DeviceGuard g(h->device);
   h->n_mels = 0;                               // not usable until the copy is complete
-  ACUDA_TRY(cudaMemcpy(h->d_basis, host_basis, sizeof(float) * n_mels * kBins, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(h->d_basis, host_basis, sizeof(float) * n_mels * kBins, cudaMemcpyHostToDevice));
   h->n_mels = n_mels;
   return LSPG_OK;
 }
 
 int lspa_logmel(lspa_handle h, const float* audio, int64_t n_samples, int n_windows, int frame_len, double step,
                 int normalize, float* out, void* stream) {
-  if (!h) return afail(LSPG_EINVAL, "null handle");
-  if (n_samples < 0) return afail(LSPG_EINVAL, "n_samples must be >= 0 (got %lld)", static_cast<long long>(n_samples));
-  if (n_windows < 0) return afail(LSPG_EINVAL, "n_windows must be >= 0 (got %d)", n_windows);
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (n_samples < 0) return fail(LSPG_EINVAL, "n_samples must be >= 0 (got %lld)", static_cast<long long>(n_samples));
+  if (n_windows < 0) return fail(LSPG_EINVAL, "n_windows must be >= 0 (got %d)", n_windows);
   if (frame_len < kMinFrame || frame_len > kMaxFrame)
-    return afail(LSPG_EINVAL, "frame_len must be in [%d, %d] (got %d): the reflect pad of %d needs a longer clip and one stft "
+    return fail(LSPG_EINVAL, "frame_len must be in [%d, %d] (got %d): the reflect pad of %d needs a longer clip and one stft "
                  "frame a shorter one", kMinFrame, kMaxFrame, frame_len, kPad);
   if (!(step >= 0.0) || !(step * static_cast<double>(n_windows) < 4.0e18))
-    return afail(LSPG_EINVAL, "step must be finite and >= 0, with n_windows * step < 4e18 (got %g)", step);
-  if ((!audio && n_samples > 0) || (!out && n_windows > 0)) return afail(LSPG_EINVAL, "null buffer");
-  if (h->device < 0) return afail(LSPG_ENODEV, "host-only handle: lspa_logmel needs an sm_90 device (no CPU path exists)");
-  if (h->n_mels == 0) return afail(LSPG_ESTATE, "lspa_load_mel_basis has not been called");
+    return fail(LSPG_EINVAL, "step must be finite and >= 0, with n_windows * step < 4e18 (got %g)", step);
+  if ((!audio && n_samples > 0) || (!out && n_windows > 0)) return fail(LSPG_EINVAL, "null buffer");
+  if (int rc = capi::require_device<Lspa>(h->device, "lspa_logmel")) return rc;
+  if (h->n_mels == 0) return fail(LSPG_ESTATE, "lspa_load_mel_basis has not been called");
   if (n_windows == 0) return LSPG_OK;
   DeviceGuard g(h->device);
   const int blocks = n_windows / kWin + (n_windows % kWin != 0);   // w0 = blockIdx.x * kWin < n_windows < 2^31
   lspa_logmel_kernel<<<blocks, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
       audio, n_samples, n_windows, frame_len, step, h->d_tw, h->d_hann, h->d_basis, h->n_mels, normalize ? 1 : 0, out);
-  ACUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
 }
 

@@ -8,7 +8,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -23,30 +22,18 @@
 
 #include "../../include/lspg.h"
 #include "aux_kernels.cuh"
+#include "capi.cuh"
 #include "raster.cuh"
 #include "conv_wgmma.cuh"
+
+using capi::DeviceGuard;
 
 namespace {
 
 using namespace lspg;
 
-thread_local std::string g_err;
-
-int fail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_err = buf;
-  return code;
-}
-
-#define CUDA_TRY(expr)                                                                         \
-  do {                                                                                         \
-    cudaError_t _e = (expr);                                                                   \
-    if (_e != cudaSuccess) return fail(LSPG_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
+struct Lspg;
+constexpr auto fail = capi::fail<Lspg>;
 
 enum Kind { K_HEAD = 0, K_S1 = 1, K_S2 = 2, K_UP = 3, K_TAIL = 4 };
 
@@ -928,7 +915,7 @@ int update_graph_io(lspg_ctx* h, Plan* P, const IoKey& io) {
 // ====================================================================================================
 extern "C" {
 
-const char* lspg_last_error(void) { return g_err.c_str(); }
+const char* lspg_last_error(void) { return capi::last_error<Lspg>().c_str(); }
 
 int lspg_create(lspg_handle* out, int variant, int ngf, int num_downs, int in_nc, int out_nc, int device) {
   if (!out) return fail(LSPG_EINVAL, "out is NULL");
@@ -941,18 +928,11 @@ int lspg_create(lspg_handle* out, int variant, int ngf, int num_downs, int in_nc
   if (out_nc != 3) return fail(LSPG_EINVAL, "out_nc must be 3 (got %d)", out_nc);
   std::unique_ptr<lspg_ctx> h(new lspg_ctx);
   h->variant = variant; h->ngf = ngf; h->num_downs = num_downs; h->in_nc = in_nc; h->out_nc = out_nc; h->device = device;
+  cudaDeviceProp prop;
+  if (int rc = capi::check_device<Lspg>(device, &prop)) return rc;
   if (device >= 0) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) return fail(LSPG_ENODEV, "no CUDA device: %s", cudaGetErrorString(e));
-    if (device >= count) return fail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0)
-      return fail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device,
-                  prop.major, prop.minor);
     h->num_sms = prop.multiProcessorCount;
-    CUDA_TRY(cudaSetDevice(device));
+    DeviceGuard g(device);
     void* fn = nullptr;
     cudaDriverEntryPointQueryResult qres;
     CUDA_TRY(cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &qres));
@@ -968,7 +948,7 @@ int lspg_create(lspg_handle* out, int variant, int ngf, int num_downs, int in_nc
 int lspg_destroy(lspg_handle h) {
   if (!h) return LSPG_OK;
   if (h->device >= 0) {
-    cudaSetDevice(h->device);
+    DeviceGuard g(h->device);
     for (auto& L : h->layers) {
       if (L.d_w) cudaFree(L.d_w);
       if (L.d_w_fast) cudaFree(L.d_w_fast);
@@ -988,21 +968,14 @@ int lspg_destroy(lspg_handle h) {
 
 int lspg_load_weights(lspg_handle h, const lspg_tensor* tensors, int n) {
   if (!h || (!tensors && n > 0)) return fail(LSPG_EINVAL, "null argument");
-  if (h->device >= 0) CUDA_TRY(cudaSetDevice(h->device));
-  std::map<std::string, const lspg_tensor*> by_name;
-  for (int i = 0; i < n; ++i) {
-    if (!tensors[i].name || !tensors[i].data) return fail(LSPG_EINVAL, "tensor %d has a null name or data pointer", i);
-    std::string nm = tensors[i].name;
-    if (nm.rfind("module.", 0) == 0) nm = nm.substr(7);   // DataParallel prefix (base_model.py:213-215)
-    by_name[nm] = &tensors[i];
-  }
+  capi::WeightTable<Lspg> wt(tensors, n);
+  if (int rc = wt.status()) return rc;
+  DeviceGuard g(h->device);
   auto take = [&](const std::string& key, std::vector<float>& dst, size_t expect, bool* changed) -> int {
-    auto it = by_name.find(key);
-    if (it == by_name.end()) return LSPG_OK;   // strict=False
-    if (static_cast<size_t>(it->second->numel) != expect)
-      return fail(LSPG_EINVAL, "%s has %lld elements, expected %zu", key.c_str(), static_cast<long long>(it->second->numel), expect);
-    if (dst.size() == expect && memcmp(dst.data(), it->second->data, expect * sizeof(float)) == 0) return LSPG_OK;
-    dst.assign(it->second->data, it->second->data + expect);
+    const float* src = wt.get(key, expect, /*required=*/false);   // strict=False: a missing key keeps what is loaded
+    if (!src) return wt.status();
+    if (dst.size() == expect && memcmp(dst.data(), src, expect * sizeof(float)) == 0) return LSPG_OK;
+    dst.assign(src, src + expect);
     *changed = true;
     return LSPG_OK;
   };
@@ -1012,7 +985,7 @@ int lspg_load_weights(lspg_handle h, const lspg_tensor* tensors, int n) {
     bool changed = false;
     int rc;
     if (L.w.empty()) { L.w.assign(wn, 0.0f); changed = true; }
-    if (by_name.count(L.conv_key + ".weight")) L.has_w = true;
+    if (wt.find(L.conv_key + ".weight")) L.has_w = true;
     if ((rc = take(L.conv_key + ".weight", L.w, wn, &changed))) return rc;
     if (L.has_bn) {
       if (L.bn_w.empty()) { L.bn_w.assign(L.cout, 1.f); L.bn_b.assign(L.cout, 0.f); L.bn_m.assign(L.cout, 0.f); L.bn_v.assign(L.cout, 1.f); }
@@ -1046,7 +1019,7 @@ static int forward_impl(lspg_handle h, const float* feature_map, int64_t fm_bstr
                         void* out, int out_is_u8, int batch, int height, int width, void* workspace, size_t workspace_bytes_in,
                         int mode, void* stream) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
-  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle: lspg_forward needs an sm_90 device (no CPU path exists)");
+  if (int rc = capi::require_device<Lspg>(h->device, "lspg_forward")) return rc;
   if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspg_load_weights has not been called");
   for (const auto& L : h->layers)
     if (!L.has_w)
@@ -1057,7 +1030,7 @@ static int forward_impl(lspg_handle h, const float* feature_map, int64_t fm_bstr
   if (rc) return rc;
   const size_t need = workspace_bytes(h, batch, height, width, mode);
   if (workspace_bytes_in < need) return fail(LSPG_ESTATE, "workspace too small: %zu < %zu", workspace_bytes_in, need);
-  CUDA_TRY(cudaSetDevice(h->device));
+  DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const auto key = std::make_tuple(batch, height, width, mode, workspace);
   auto it = h->plans.find(key);
@@ -1119,8 +1092,8 @@ int lspg_draw_feature_maps(lspg_handle h, const float* landmarks, const float* s
   if (batch <= 0 || height <= 0 || width <= 0) return fail(LSPG_EINVAL, "bad shape %d x %d x %d", batch, height, width);
   if (shoulders != nullptr && (n_shoulder_points < 0 || n_shoulder_points % 2 != 0))
     return fail(LSPG_EINVAL, "n_shoulder_points must be even (two polylines), got %d", n_shoulder_points);
-  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle: lspg_draw_feature_maps needs an sm_90 device (no CPU path exists)");
-  CUDA_TRY(cudaSetDevice(h->device));
+  if (int rc = capi::require_device<Lspg>(h->device, "lspg_draw_feature_maps")) return rc;
+  DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   CUDA_TRY(cudaMemsetAsync(out_fm, 0, sizeof(float) * static_cast<size_t>(batch) * height * width, st));
   const int n_sh = shoulders ? n_shoulder_points : 0;
@@ -1198,7 +1171,7 @@ int lspg_debug_read_tensor(lspg_handle h, int id, int limb, uint16_t* dst, int64
   if (limb < 0 || limb >= nl_of(P->mode)) return fail(LSPG_EINVAL, "limb %d not present in this mode", limb);
   const size_t bytes = tensor_bytes_one_limb(h->tensors[id], P->batch, P->height, P->width);
   if (static_cast<size_t>(count) * 2 != bytes) return fail(LSPG_EINVAL, "count %lld != %zu", static_cast<long long>(count), bytes / 2);
-  CUDA_TRY(cudaSetDevice(h->device));
+  DeviceGuard g(h->device);
   CUDA_TRY(cudaDeviceSynchronize());
   CUDA_TRY(cudaMemcpy(dst, static_cast<uint8_t*>(P->workspace) + P->tensor_off[id] + limb * P->tensor_limb_stride[id], bytes,
                       cudaMemcpyDeviceToHost));
@@ -1238,7 +1211,7 @@ int lspg_debug_read_trace(lspg_handle h, uint64_t* dst, int64_t count) {
   if (!h || !dst) return fail(LSPG_EINVAL, "null argument");
   if (!h->trace_buf) return fail(LSPG_ESTATE, "no trace recorded (set LSPG_TRACE_LAYER=<layer index> before the first forward)");
   if (count != 256 * kTraceSlots) return fail(LSPG_EINVAL, "count must be %d", 256 * kTraceSlots);
-  CUDA_TRY(cudaSetDevice(h->device));
+  DeviceGuard g(h->device);
   CUDA_TRY(cudaDeviceSynchronize());
   CUDA_TRY(cudaMemcpy(dst, h->trace_buf, sizeof(uint64_t) * count, cudaMemcpyDeviceToHost));
   return LSPG_OK;
@@ -1253,7 +1226,7 @@ int lspg_graph_stats(lspg_handle h, int64_t* captures, int64_t* io_updates, int6
 int lspg_release_workspace(lspg_handle h, void* workspace) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
   if (h->device >= 0) {
-    CUDA_TRY(cudaSetDevice(h->device));
+    DeviceGuard g(h->device);
     CUDA_TRY(cudaDeviceSynchronize());            // forwards that still use the workspace finish before their plan goes
   }
   for (auto it = h->plans.begin(); it != h->plans.end();) {
@@ -1279,7 +1252,7 @@ int lspg_launches_per_forward(lspg_handle h, int* out) {
 
 int lspg_profile_enable(lspg_handle h, int enabled) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
-  if (h->device < 0) return fail(LSPG_ENODEV, "host-only handle");
+  if (int rc = capi::require_device<Lspg>(h->device, "lspg_profile_enable")) return rc;
   h->profiling = enabled != 0;
   h->prof_used = 0;
   return LSPG_OK;
@@ -1289,7 +1262,8 @@ int lspg_profile_read(lspg_handle h, float* avg_ms, int count, int* n_forwards) 
   if (!h || !avg_ms || !n_forwards) return fail(LSPG_EINVAL, "null argument");
   const int n = 1 + static_cast<int>(h->layers.size());
   if (count != n) return fail(LSPG_EINVAL, "count %d != launches per forward %d", count, n);
-  CUDA_TRY(cudaSetDevice(h->device));
+  if (int rc = capi::require_device<Lspg>(h->device, "lspg_profile_read")) return rc;
+  DeviceGuard g(h->device);
   for (int i = 0; i < n; ++i) avg_ms[i] = 0.f;
   for (size_t f = 0; f < h->prof_used; ++f) {
     auto& set = h->prof_events[f];

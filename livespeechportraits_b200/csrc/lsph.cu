@@ -25,38 +25,22 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <cstring>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/lsph.h"
+#include "capi.cuh"
 #include "gemm_nt.cuh"
 
 namespace cg = cooperative_groups;
+using capi::DeviceGuard;
 
 namespace {
 
-thread_local std::string g_herr;
-
-int hfail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_herr = buf;
-  return code;
-}
-
-#define HCUDA_TRY(expr)                                                                           \
-  do {                                                                                            \
-    cudaError_t _e = (expr);                                                                      \
-    if (_e != cudaSuccess) return hfail(LSPG_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
+struct Lsph;
+constexpr auto fail = capi::fail<Lsph>;
 
 constexpr int kR = 128;          // residual = dilation channels
 constexpr int kS = 256;          // skip channels
@@ -369,10 +353,10 @@ namespace {
 int upload(lsph_ctx* h, float** dst, const std::vector<float>& src) {
   if (h->device < 0) return LSPG_OK;
   if (!*dst) {
-    HCUDA_TRY(cudaMalloc(dst, src.size() * sizeof(float)));
+    CUDA_TRY(cudaMalloc(dst, src.size() * sizeof(float)));
     h->owned.push_back(*dst);
   }
-  HCUDA_TRY(cudaMemcpy(*dst, src.data(), src.size() * sizeof(float), cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(*dst, src.data(), src.size() * sizeof(float), cudaMemcpyHostToDevice));
   return LSPG_OK;
 }
 
@@ -380,44 +364,37 @@ int upload(lsph_ctx* h, float** dst, const std::vector<float>& src) {
 
 extern "C" {
 
-const char* lsph_last_error(void) { return g_herr.c_str(); }
+const char* lsph_last_error(void) { return capi::last_error<Lsph>().c_str(); }
 
 int lsph_create(lsph_handle* out, const lsph_config* c, int device) {
-  if (!out || !c) return hfail(LSPG_EINVAL, "null argument");
+  if (!out || !c) return fail(LSPG_EINVAL, "null argument");
   *out = nullptr;
-  if (c->residual_ch != kR || c->dilation_ch != kR) return hfail(LSPG_EINVAL, "residual/dilation channels must be %d (got %d/%d)", kR, c->residual_ch, c->dilation_ch);
-  if (c->skip_ch != kS) return hfail(LSPG_EINVAL, "skip channels must be %d (got %d)", kS, c->skip_ch);
-  if (c->kernel_size != 2) return hfail(LSPG_EINVAL, "kernel_size must be 2 (got %d)", c->kernel_size);
-  if (c->layers < 1 || c->blocks < 1 || c->layers * c->blocks > kMaxLayers || c->layers > 20) return hfail(LSPG_EINVAL, "layers x blocks out of range");
-  if (c->input_ch < 1 || c->input_ch > kMaxIn) return hfail(LSPG_EINVAL, "input_ch out of range [1,%d]", kMaxIn);
-  if (c->ndim < 1 || c->ncenter < 1) return hfail(LSPG_EINVAL, "bad GMM shape");
-  if (c->ndim != c->input_ch) return hfail(LSPG_EINVAL, "ndim (%d) must equal input_ch (%d): the sample is fed back as the next input", c->ndim, c->input_ch);
+  if (c->residual_ch != kR || c->dilation_ch != kR) return fail(LSPG_EINVAL, "residual/dilation channels must be %d (got %d/%d)", kR, c->residual_ch, c->dilation_ch);
+  if (c->skip_ch != kS) return fail(LSPG_EINVAL, "skip channels must be %d (got %d)", kS, c->skip_ch);
+  if (c->kernel_size != 2) return fail(LSPG_EINVAL, "kernel_size must be 2 (got %d)", c->kernel_size);
+  if (c->layers < 1 || c->blocks < 1 || c->layers * c->blocks > kMaxLayers || c->layers > 20) return fail(LSPG_EINVAL, "layers x blocks out of range");
+  if (c->input_ch < 1 || c->input_ch > kMaxIn) return fail(LSPG_EINVAL, "input_ch out of range [1,%d]", kMaxIn);
+  if (c->ndim < 1 || c->ncenter < 1) return fail(LSPG_EINVAL, "bad GMM shape");
+  if (c->ndim != c->input_ch) return fail(LSPG_EINVAL, "ndim (%d) must equal input_ch (%d): the sample is fed back as the next input", c->ndim, c->input_ch);
   const int O = c->loss_gmm ? (2 * c->ndim + 1) * c->ncenter : c->ndim;
-  if (O > kMaxOut) return hfail(LSPG_EINVAL, "output size %d exceeds %d", O, kMaxOut);
+  if (O > kMaxOut) return fail(LSPG_EINVAL, "output size %d exceeds %d", O, kMaxOut);
   if (c->apc_hidden < 64 || c->apc_hidden % 64 || c->cond_ch != c->apc_hidden)
-    return hfail(LSPG_EINVAL, "apc_hidden must be a multiple of 64 and equal cond_ch (got %d / %d)", c->apc_hidden, c->cond_ch);
-  if (c->frame_future < 0) return hfail(LSPG_EINVAL, "frame_future must be >= 0");
+    return fail(LSPG_EINVAL, "apc_hidden must be a multiple of 64 and equal cond_ch (got %d / %d)", c->apc_hidden, c->cond_ch);
+  if (c->frame_future < 0) return fail(LSPG_EINVAL, "frame_future must be >= 0");
   std::unique_ptr<lsph_ctx> h(new lsph_ctx);
   h->cfg = *c; h->device = device; h->O = O;
   h->L = c->layers * c->blocks;
   h->rf = 1;
   for (int b = 0; b < c->blocks; ++b)
     for (int i = 0; i < c->layers; ++i) { h->dil.push_back(1 << i); h->rf += (1 << i); }      // networks.py:160-176
-  if (device >= 0) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) return hfail(LSPG_ENODEV, "no CUDA device: %s", cudaGetErrorString(e));
-    if (device >= count) return hfail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
-    cudaDeviceProp prop;
-    HCUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) return hfail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device, prop.major, prop.minor);
-  }
+  cudaDeviceProp prop;
+  if (int rc = capi::check_device<Lsph>(device, &prop)) return rc;
   *out = h.release();
   return LSPG_OK;
 }
 
 int lsph_receptive_field(lsph_handle h, int* out) {
-  if (!h || !out) return hfail(LSPG_EINVAL, "null argument");
+  if (!h || !out) return fail(LSPG_EINVAL, "null argument");
   *out = h->rf;
   return LSPG_OK;
 }
@@ -425,7 +402,7 @@ int lsph_receptive_field(lsph_handle h, int* out) {
 int lsph_destroy(lsph_handle h) {
   if (!h) return LSPG_OK;
   if (h->device >= 0) {
-    cudaSetDevice(h->device);
+    DeviceGuard g(h->device);
     for (float* p : h->owned) cudaFree(p);
     for (float* p : {h->d_ds1, h->d_ds2, h->d_cond, h->d_hist})
       if (p) cudaFree(p);
@@ -435,47 +412,29 @@ int lsph_destroy(lsph_handle h) {
 }
 
 int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n) {
-  if (!h || (!tensors && n > 0)) return hfail(LSPG_EINVAL, "null argument");
+  if (!h || (!tensors && n > 0)) return fail(LSPG_EINVAL, "null argument");
   const lsph_config& c = h->cfg;
-  std::map<std::string, const lspg_tensor*> by_name;
-  for (int i = 0; i < n; ++i) {
-    if (!tensors[i].name || !tensors[i].data) return hfail(LSPG_EINVAL, "tensor %d has a null name or data pointer", i);
-    std::string nm = tensors[i].name;
-    if (nm.rfind("module.", 0) == 0) nm = nm.substr(7);
-    by_name[nm] = &tensors[i];
-  }
-  int rc = LSPG_OK;
-  auto get = [&](const std::string& key, size_t expect, bool required = true) -> const float* {
-    auto it = by_name.find(key);
-    if (it == by_name.end()) {
-      if (required && rc == LSPG_OK) rc = hfail(LSPG_ESTATE, "missing parameter %s", key.c_str());
-      return nullptr;
-    }
-    if (static_cast<size_t>(it->second->numel) != expect) {
-      if (rc == LSPG_OK) rc = hfail(LSPG_EINVAL, "%s has %lld elements, expected %zu", key.c_str(), static_cast<long long>(it->second->numel), expect);
-      return nullptr;
-    }
-    return it->second->data;
-  };
+  capi::WeightTable<Lsph> wt(tensors, n);
+  if (int rc = wt.status()) return rc;
   const int H = c.apc_hidden, C = c.cond_ch, I = c.input_ch, O = h->O, L = h->L;
   // ---- audio_downsample (models/audio2headpose.py:17-22): Linear - BatchNorm1d(eval) - LeakyReLU - Linear
-  const float* w0 = get("audio_downsample.0.weight", static_cast<size_t>(H) * 2 * H);
-  const float* b0 = get("audio_downsample.0.bias", H);
-  const float* bw = get("audio_downsample.1.weight", H);
-  const float* bb = get("audio_downsample.1.bias", H);
-  const float* bm = get("audio_downsample.1.running_mean", H);
-  const float* bv = get("audio_downsample.1.running_var", H);
-  const float* w3 = get("audio_downsample.3.weight", static_cast<size_t>(H) * H);
-  const float* b3 = get("audio_downsample.3.bias", H);
-  const float* ws1 = get("WaveNet.start_conv1.weight", static_cast<size_t>(kR) * I);
-  const float* bs1 = get("WaveNet.start_conv1.bias", kR);
-  const float* ws2 = get("WaveNet.start_conv2.weight", static_cast<size_t>(kR) * kR);
-  const float* bs2 = get("WaveNet.start_conv2.bias", kR);
-  const float* we1 = get("WaveNet.end_conv_1.weight", static_cast<size_t>(O) * kS);
-  const float* be1 = get("WaveNet.end_conv_1.bias", O);
-  const float* we2 = get("WaveNet.end_conv_2.weight", static_cast<size_t>(O) * O);
-  const float* be2 = get("WaveNet.end_conv_2.bias", O);
-  if (rc) return rc;
+  const float* w0 = wt.get("audio_downsample.0.weight", static_cast<size_t>(H) * 2 * H);
+  const float* b0 = wt.get("audio_downsample.0.bias", H);
+  const float* bw = wt.get("audio_downsample.1.weight", H);
+  const float* bb = wt.get("audio_downsample.1.bias", H);
+  const float* bm = wt.get("audio_downsample.1.running_mean", H);
+  const float* bv = wt.get("audio_downsample.1.running_var", H);
+  const float* w3 = wt.get("audio_downsample.3.weight", static_cast<size_t>(H) * H);
+  const float* b3 = wt.get("audio_downsample.3.bias", H);
+  const float* ws1 = wt.get("WaveNet.start_conv1.weight", static_cast<size_t>(kR) * I);
+  const float* bs1 = wt.get("WaveNet.start_conv1.bias", kR);
+  const float* ws2 = wt.get("WaveNet.start_conv2.weight", static_cast<size_t>(kR) * kR);
+  const float* bs2 = wt.get("WaveNet.start_conv2.bias", kR);
+  const float* we1 = wt.get("WaveNet.end_conv_1.weight", static_cast<size_t>(O) * kS);
+  const float* be1 = wt.get("WaveNet.end_conv_1.bias", O);
+  const float* we2 = wt.get("WaveNet.end_conv_2.weight", static_cast<size_t>(O) * O);
+  const float* be2 = wt.get("WaveNet.end_conv_2.bias", O);
+  if (int rc = wt.status()) return rc;
   std::vector<float> scale0(H), shift0(H), one(std::max(H, L * 2 * kR), 1.0f);
   for (int j = 0; j < H; ++j) {
     const float s = bw[j] / sqrtf(bv[j] + 1e-5f);          // BatchNorm1d eval, eps = torch default
@@ -486,19 +445,19 @@ int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n) {
   std::vector<float> w_cond(static_cast<size_t>(L) * 2 * kR * C), b_cond(static_cast<size_t>(L) * 2 * kR, 0.f);
   for (int l = 0; l < L; ++l) {
     const std::string p = "WaveNet.residual_blocks." + std::to_string(l) + ".";
-    const float* wf = get(p + "filter_conv.weight", static_cast<size_t>(kR) * kR * 2);
-    const float* wg = get(p + "gate_conv.weight", static_cast<size_t>(kR) * kR * 2);
-    const float* wr = get(p + "residual_conv.weight", static_cast<size_t>(kR) * kR);
-    const float* wsk = get(p + "skip_conv.weight", static_cast<size_t>(kS) * kR);
-    const float* wcf = get(p + "cond_filter_conv.weight", static_cast<size_t>(kR) * C);
-    const float* wcg = get(p + "cond_gate_conv.weight", static_cast<size_t>(kR) * C);
-    const float* bcf = get(p + "cond_filter_conv.bias", kR);
-    const float* bcg = get(p + "cond_gate_conv.bias", kR);
-    const float* bf = get(p + "filter_conv.bias", kR, c.use_bias != 0);
-    const float* bg = get(p + "gate_conv.bias", kR, c.use_bias != 0);
-    const float* br = get(p + "residual_conv.bias", kR, c.use_bias != 0);
-    const float* bsk = get(p + "skip_conv.bias", kS, c.use_bias != 0);
-    if (rc) return rc;
+    const float* wf = wt.get(p + "filter_conv.weight", static_cast<size_t>(kR) * kR * 2);
+    const float* wg = wt.get(p + "gate_conv.weight", static_cast<size_t>(kR) * kR * 2);
+    const float* wr = wt.get(p + "residual_conv.weight", static_cast<size_t>(kR) * kR);
+    const float* wsk = wt.get(p + "skip_conv.weight", static_cast<size_t>(kS) * kR);
+    const float* wcf = wt.get(p + "cond_filter_conv.weight", static_cast<size_t>(kR) * C);
+    const float* wcg = wt.get(p + "cond_gate_conv.weight", static_cast<size_t>(kR) * C);
+    const float* bcf = wt.get(p + "cond_filter_conv.bias", kR);
+    const float* bcg = wt.get(p + "cond_gate_conv.bias", kR);
+    const float* bf = wt.get(p + "filter_conv.bias", kR, c.use_bias != 0);
+    const float* bg = wt.get(p + "gate_conv.bias", kR, c.use_bias != 0);
+    const float* br = wt.get(p + "residual_conv.bias", kR, c.use_bias != 0);
+    const float* bsk = wt.get(p + "skip_conv.bias", kS, c.use_bias != 0);
+    if (int rc = wt.status()) return rc;
     // conv1d weight [out][in][tap]; tap 0 multiplies x[t - d], tap 1 multiplies x[t] (left zero padding, networks.py:271,307)
     for (int o = 0; o < kR; ++o)
       for (int k = 0; k < kR; ++k)
@@ -518,10 +477,8 @@ int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n) {
     if (bsk)
       for (int o = 0; o < kS; ++o) b_rs[static_cast<size_t>(l) * (kR + kS) + kR + o] = bsk[o];
   }
-  if (h->device >= 0) {
-    HCUDA_TRY(cudaSetDevice(h->device));
-    HCUDA_TRY(cudaDeviceSynchronize());
-  }
+  DeviceGuard g(h->device);
+  if (h->device >= 0) CUDA_TRY(cudaDeviceSynchronize());
   auto vec = [](const float* p, size_t n) { return std::vector<float>(p, p + n); };
   int r2;
   if ((r2 = upload(h, &h->d_w_ds0, vec(w0, static_cast<size_t>(H) * 2 * H)))) return r2;
@@ -550,39 +507,39 @@ int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n) {
 }
 
 int lsph_debug_packed(lsph_handle h, int which, float* dst, int64_t count) {
-  if (!h || !dst) return hfail(LSPG_EINVAL, "null argument");
-  if (which < 0 || which > 6) return hfail(LSPG_EINVAL, "which must be 0..6");
-  if (!h->weights_loaded) return hfail(LSPG_ESTATE, "weights not loaded");
+  if (!h || !dst) return fail(LSPG_EINVAL, "null argument");
+  if (which < 0 || which > 6) return fail(LSPG_EINVAL, "which must be 0..6");
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "weights not loaded");
   if (static_cast<size_t>(count) != h->packed[which].size())
-    return hfail(LSPG_EINVAL, "count %lld != %zu", static_cast<long long>(count), h->packed[which].size());
+    return fail(LSPG_EINVAL, "count %lld != %zu", static_cast<long long>(count), h->packed[which].size());
   memcpy(dst, h->packed[which].data(), sizeof(float) * h->packed[which].size());
   return LSPG_OK;
 }
 
 int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
                   const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream) {
-  if (!h) return hfail(LSPG_EINVAL, "null handle");
-  if (h->device < 0) return hfail(LSPG_ENODEV, "host-only handle: lsph_generate needs an sm_90 device (no CPU path exists)");
-  if (!h->weights_loaded) return hfail(LSPG_ESTATE, "lsph_load_weights has not been called");
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (int rc = capi::require_device<Lsph>(h->device, "lsph_generate")) return rc;
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lsph_load_weights has not been called");
   const lsph_config& c = h->cfg;
-  if (!audio_feats || !pre_headpose || !out_pred) return hfail(LSPG_EINVAL, "null buffer");
-  if (c.loss_gmm && !noise) return hfail(LSPG_EINVAL, "noise is required for the GMM loss (pass zeros for sigma_scale 0)");
+  if (!audio_feats || !pre_headpose || !out_pred) return fail(LSPG_EINVAL, "null buffer");
+  if (c.loss_gmm && !noise) return fail(LSPG_EINVAL, "noise is required for the GMM loss (pass zeros for sigma_scale 0)");
   const int nframe = n_audio - c.frame_future;
-  if (nframe < 1) return hfail(LSPG_EINVAL, "need more than frame_future (%d) audio rows, got %d", c.frame_future, n_audio);
+  if (nframe < 1) return fail(LSPG_EINVAL, "need more than frame_future (%d) audio rows, got %d", c.frame_future, n_audio);
   if (cluster == 0) cluster = 8;
-  if (cluster != 1 && cluster != 8) return hfail(LSPG_EINVAL, "cluster must be 1 or 8 (got %d)", cluster);
-  HCUDA_TRY(cudaSetDevice(h->device));
+  if (cluster != 1 && cluster != 8) return fail(LSPG_EINVAL, "cluster must be 1 or 8 (got %d)", cluster);
+  DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int H = c.apc_hidden, L = h->L, T = h->rf - 1 + nframe;
   if (n_audio > h->cap_audio) {
-    HCUDA_TRY(cudaDeviceSynchronize());
+    CUDA_TRY(cudaDeviceSynchronize());
     for (float** p : {&h->d_ds1, &h->d_ds2, &h->d_cond, &h->d_hist})
       if (*p) { cudaFree(*p); *p = nullptr; }
     const int cap = n_audio + 64;
-    HCUDA_TRY(cudaMalloc(&h->d_ds1, sizeof(float) * static_cast<size_t>(cap) * H));
-    HCUDA_TRY(cudaMalloc(&h->d_ds2, sizeof(float) * static_cast<size_t>(cap) * H));
-    HCUDA_TRY(cudaMalloc(&h->d_cond, sizeof(float) * static_cast<size_t>(cap) * L * 2 * kR));
-    HCUDA_TRY(cudaMalloc(&h->d_hist, sizeof(float) * static_cast<size_t>(L) * (h->rf - 1 + cap) * kR));
+    CUDA_TRY(cudaMalloc(&h->d_ds1, sizeof(float) * static_cast<size_t>(cap) * H));
+    CUDA_TRY(cudaMalloc(&h->d_ds2, sizeof(float) * static_cast<size_t>(cap) * H));
+    CUDA_TRY(cudaMalloc(&h->d_cond, sizeof(float) * static_cast<size_t>(cap) * L * 2 * kR));
+    CUDA_TRY(cudaMalloc(&h->d_hist, sizeof(float) * static_cast<size_t>(L) * (h->rf - 1 + cap) * kR));
     h->cap_audio = cap;
   }
   // ---- hoisted audio path: downsample every row, project it for every block
@@ -591,7 +548,7 @@ int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const fl
   gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, h->d_ds1, n_audio, H, 2 * H, 1, 0);
   gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(h->d_ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, h->d_ds2, n_audio, H, H, 0, 0);
   gemm_nt_kernel<><<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(h->d_ds2, h->d_w_cond, h->d_one, h->d_b_cond, h->d_cond, n_audio, L * 2 * kR, H, 0, 0);
-  HCUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   LoopParams p;
   memset(&p, 0, sizeof(p));
   p.w_start1 = h->d_w_start1; p.b_start1 = h->d_b_start1; p.w_start2 = h->d_w_start2; p.b_start2 = h->d_b_start2;
@@ -610,10 +567,10 @@ int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const fl
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = 8; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    HCUDA_TRY(cudaLaunchKernelEx(&cfg, headpose_loop_kernel<8, 16>, p));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, headpose_loop_kernel<8, 16>, p));
   } else {
     headpose_loop_kernel<1, 32><<<1, 32 * 32, 0, st>>>(p);
-    HCUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
   }
   return LSPG_OK;
 }

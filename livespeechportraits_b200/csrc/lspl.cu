@@ -22,31 +22,16 @@
 #include <cuda_runtime.h>
 
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
-#include <string>
 
 #include "../../include/lspl.h"
+#include "capi.cuh"
+
+using capi::DeviceGuard;
 
 namespace {
 
-thread_local std::string g_lerr;
-
-int lfail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_lerr = buf;
-  return code;
-}
-
-#define LCUDA_TRY(expr)                                                                           \
-  do {                                                                                            \
-    cudaError_t _e = (expr);                                                                      \
-    if (_e != cudaSuccess) return lfail(LSPG_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
+struct Lspl;
+constexpr auto fail = capi::fail<Lspl>;
 
 constexpr int kPts = 73;
 constexpr int kMouth0 = 46;                    // rows 46..63 of the face come from the mouth track
@@ -330,14 +315,6 @@ __global__ void __launch_bounds__(kThreads) lspl_project_kernel(int nframe, int 
   }
 }
 
-class DeviceGuard {
- public:
-  explicit DeviceGuard(int dev) { cudaGetDevice(&prev_); if (prev_ != dev) cudaSetDevice(dev); dev_ = dev; }
-  ~DeviceGuard() { if (prev_ != dev_) cudaSetDevice(prev_); }
- private:
-  int prev_ = 0, dev_ = 0;
-};
-
 }  // namespace
 
 struct lspl_ctx {
@@ -349,7 +326,7 @@ struct lspl_ctx {
 
 extern "C" {
 
-const char* lspl_last_error(void) { return g_lerr.c_str(); }
+const char* lspl_last_error(void) { return capi::last_error<Lspl>().c_str(); }
 
 int lspl_destroy(lspl_handle h) {
   if (!h) return LSPG_OK;
@@ -363,19 +340,10 @@ int lspl_destroy(lspl_handle h) {
 }
 
 int lspl_create(lspl_handle* out, int device) {
-  if (!out) return lfail(LSPG_EINVAL, "null argument");
+  if (!out) return fail(LSPG_EINVAL, "null argument");
   *out = nullptr;
-  if (device < -1) return lfail(LSPG_EINVAL, "device must be >= -1 (got %d)", device);
-  if (device >= 0) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) return lfail(LSPG_ENODEV, "no CUDA device: %s", cudaGetErrorString(e));
-    if (device >= count) return lfail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
-    cudaDeviceProp prop;
-    LCUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0)
-      return lfail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device, prop.major, prop.minor);
-  }
+  cudaDeviceProp prop;
+  if (int rc = capi::check_device<Lspl>(device, &prop)) return rc;
   lspl_ctx* h = new lspl_ctx;
   h->device = device;
   if (device >= 0) {
@@ -383,7 +351,7 @@ int lspl_create(lspl_handle* out, int device) {
     cudaError_t e = cudaMalloc(&h->d_id, sizeof(DevIdentity));
     if (e != cudaSuccess) {
       lspl_destroy(h);
-      return lfail(LSPG_ECUDA, "lspl_create: %s", cudaGetErrorString(e));
+      return fail(LSPG_ECUDA, "lspl_create: %s", cudaGetErrorString(e));
     }
   }
   *out = h;
@@ -391,11 +359,11 @@ int lspl_create(lspl_handle* out, int device) {
 }
 
 int lspl_load_identity(lspl_handle h, const lspl_identity* id) {
-  if (!h || !id) return lfail(LSPG_EINVAL, "null argument");
+  if (!h || !id) return fail(LSPG_EINVAL, "null argument");
   if (!id->mean_pts3d || !id->std_mean_pts3d || !id->candidate_eye_brow || !id->shoulder3D)
-    return lfail(LSPG_EINVAL, "null identity array");
-  if (id->n_candidates < 1) return lfail(LSPG_EINVAL, "n_candidates must be >= 1 (got %d)", id->n_candidates);
-  if (h->device < 0) return lfail(LSPG_ENODEV, "host-only handle: lspl_load_identity needs an sm_90 device (no CPU path exists)");
+    return fail(LSPG_EINVAL, "null identity array");
+  if (id->n_candidates < 1) return fail(LSPG_EINVAL, "n_candidates must be >= 1 (got %d)", id->n_candidates);
+  if (int rc = capi::require_device<Lspl>(h->device, "lspl_load_identity")) return rc;
   static const int brow_rows[16] = {27, 65, 28, 68, 29, 67, 30, 66, 31, 72, 32, 69, 33, 70, 34, 71};
   DevIdentity d{};
   for (int i = 0; i < kMouthCols; ++i) d.mouth_mean[i] = id->mean_pts3d[kMouth0 * 3 + i];
@@ -429,15 +397,15 @@ int lspl_load_identity(lspl_handle h, const lspl_identity* id) {
   if (e == cudaSuccess) e = cudaMemcpy(h->d_brow, brow, sizeof(float) * 48 * static_cast<size_t>(m), cudaMemcpyHostToDevice);
   if (e == cudaSuccess) e = cudaMemcpy(h->d_id, &d, sizeof(d), cudaMemcpyHostToDevice);
   delete[] brow;
-  if (e != cudaSuccess) return lfail(LSPG_ECUDA, "lspl_load_identity: %s", cudaGetErrorString(e));
+  if (e != cudaSuccess) return fail(LSPG_ECUDA, "lspl_load_identity: %s", cudaGetErrorString(e));
   h->n_brow = m;
   return LSPG_OK;
 }
 
 int lspl_workspace_bytes(lspl_handle h, int n_feat, int n_head, size_t* out) {
-  if (!h || !out) return lfail(LSPG_EINVAL, "null argument");
+  if (!h || !out) return fail(LSPG_EINVAL, "null argument");
   if (n_feat < 0 || n_head < 0 || n_feat > kMaxN || n_head > kMaxN)
-    return lfail(LSPG_EINVAL, "track lengths must be in [0, 2^29] (got %d, %d)", n_feat, n_head);
+    return fail(LSPG_EINVAL, "track lengths must be in [0, 2^29] (got %d, %d)", n_feat, n_head);
   carve(nullptr, n_feat < n_head ? n_feat : n_head, out);
   return LSPG_OK;
 }
@@ -445,28 +413,28 @@ int lspl_workspace_bytes(lspl_handle h, int n_feat, int n_head, size_t* out) {
 int lspl_run(lspl_handle h, const float* pred_feat, int n_feat, const float* pred_head, int n_head, int head_stride,
              const lspl_params* p, float* landmarks, float* shoulders, float* final_pts3d, float* pred_headpose,
              void* workspace, size_t workspace_bytes, void* stream) {
-  if (!h || !p) return lfail(LSPG_EINVAL, "null argument");
+  if (!h || !p) return fail(LSPG_EINVAL, "null argument");
   if (n_feat < 0 || n_head < 0 || n_feat > kMaxN || n_head > kMaxN)
-    return lfail(LSPG_EINVAL, "track lengths must be in [0, 2^29] (got %d, %d)", n_feat, n_head);
-  if (head_stride < 6) return lfail(LSPG_EINVAL, "head_stride must be >= 6 (got %d)", head_stride);
+    return fail(LSPG_EINVAL, "track lengths must be in [0, 2^29] (got %d, %d)", n_feat, n_head);
+  if (head_stride < 6) return fail(LSPG_EINVAL, "head_stride must be >= 6 (got %d)", head_stride);
   if (!(p->feat_sigma >= 0.0) || radius_of(p->feat_sigma) > LSPL_MAX_RADIUS)
-    return lfail(LSPG_EINVAL, "feat_sigma must be >= 0 with int(4 sigma + 0.5) <= %d (got %g)", LSPL_MAX_RADIUS, p->feat_sigma);
+    return fail(LSPG_EINVAL, "feat_sigma must be >= 0 with int(4 sigma + 0.5) <= %d (got %g)", LSPL_MAX_RADIUS, p->feat_sigma);
   if (!(p->rot_sigma > 0.0) || !(p->trans_sigma > 0.0) || radius_of(p->rot_sigma) > LSPL_MAX_RADIUS ||
       radius_of(p->trans_sigma) > LSPL_MAX_RADIUS)
-    return lfail(LSPG_EINVAL, "head sigmas must be > 0 with int(4 sigma + 0.5) <= %d (got %g, %g): scipy's "
+    return fail(LSPG_EINVAL, "head sigmas must be > 0 with int(4 sigma + 0.5) <= %d (got %g, %g): scipy's "
                  "gaussian_filter1d divides by zero at 0", LSPL_MAX_RADIUS, p->rot_sigma, p->trans_sigma);
   const int nframe = n_feat < n_head ? n_feat : n_head;
-  if ((!pred_feat && n_feat > 0) || (!pred_head && n_head > 0)) return lfail(LSPG_EINVAL, "null input track");
-  if (nframe > 0 && (!landmarks || !shoulders)) return lfail(LSPG_EINVAL, "null output buffer");
+  if ((!pred_feat && n_feat > 0) || (!pred_head && n_head > 0)) return fail(LSPG_EINVAL, "null input track");
+  if (nframe > 0 && (!landmarks || !shoulders)) return fail(LSPG_EINVAL, "null output buffer");
   if (reinterpret_cast<uintptr_t>(landmarks) % 8 || reinterpret_cast<uintptr_t>(shoulders) % 8)
-    return lfail(LSPG_EINVAL, "landmarks and shoulders must be 8-byte aligned");
-  if (h->device < 0) return lfail(LSPG_ENODEV, "host-only handle: lspl_run needs an sm_90 device (no CPU path exists)");
-  if (h->n_brow == 0) return lfail(LSPG_ESTATE, "lspl_load_identity has not been called");
+    return fail(LSPG_EINVAL, "landmarks and shoulders must be 8-byte aligned");
+  if (int rc = capi::require_device<Lspl>(h->device, "lspl_run")) return rc;
+  if (h->n_brow == 0) return fail(LSPG_ESTATE, "lspl_load_identity has not been called");
   if (nframe == 0) return LSPG_OK;
   size_t need = 0;
   carve(nullptr, nframe, &need);
   if (!workspace || workspace_bytes < need)
-    return lfail(LSPG_ESTATE, "workspace of %zu bytes is smaller than the %zu lspl_workspace_bytes gives", workspace_bytes, need);
+    return fail(LSPG_ESTATE, "workspace of %zu bytes is smaller than the %zu lspl_workspace_bytes gives", workspace_bytes, need);
   Workspace ws = carve(workspace, nframe, &need);
   KParams kp{};
   for (int i = 0; i < kMouthCols; ++i) kp.amp[i] = p->amp[i / 3][i % 3];
@@ -486,10 +454,10 @@ int lspl_run(lspl_handle h, const float* pred_feat, int n_feat, const float* pre
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   lspl_smooth_kernel<<<ctas, kThreads, smem, st>>>(pred_feat, pred_head, nframe, n_head, head_stride, p->feat_sigma,
                                                    p->rot_sigma, p->trans_sigma, kp, h->d_id, ws, pred_headpose);
-  LCUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   lspl_project_kernel<<<ctas, kThreads, 0, st>>>(nframe, ctas, kp, h->d_id, h->d_brow, h->n_brow, ws, landmarks, shoulders,
                                                  final_pts3d);
-  LCUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
 }
 

@@ -20,31 +20,16 @@
 
 #include <climits>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
-#include <string>
 
 #include "../../include/lspm.h"
+#include "capi.cuh"
+
+using capi::DeviceGuard;
 
 namespace {
 
-thread_local std::string g_merr;
-
-int mfail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_merr = buf;
-  return code;
-}
-
-#define MCUDA_TRY(expr)                                                                           \
-  do {                                                                                            \
-    cudaError_t _e = (expr);                                                                      \
-    if (_e != cudaSuccess) return mfail(LSPG_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
+struct Lspm;
+constexpr auto fail = capi::fail<Lspm>;
 
 constexpr int kMaxK = 32;        // neighbours: one warp lane per list entry
 constexpr int kMaxDim = 1024;
@@ -369,14 +354,6 @@ size_t workspace_bytes(int n, int k) {
   return align256(sizeof(float) * n) + align256(sizeof(float) * cand) + align256(sizeof(int) * cand);
 }
 
-class DeviceGuard {
- public:
-  explicit DeviceGuard(int dev) { cudaGetDevice(&prev_); if (prev_ != dev) cudaSetDevice(dev); dev_ = dev; }
-  ~DeviceGuard() { if (prev_ != dev_) cudaSetDevice(prev_); }
- private:
-  int prev_ = 0, dev_ = 0;
-};
-
 }  // namespace
 
 struct lspm_ctx {
@@ -389,24 +366,17 @@ struct lspm_ctx {
 
 extern "C" {
 
-const char* lspm_last_error(void) { return g_merr.c_str(); }
+const char* lspm_last_error(void) { return capi::last_error<Lspm>().c_str(); }
 
 int lspm_create(lspm_handle* out, int dim, int device) {
-  if (!out) return mfail(LSPG_EINVAL, "null argument");
+  if (!out) return fail(LSPG_EINVAL, "null argument");
   *out = nullptr;
-  if (dim < 32 || dim > kMaxDim || dim % 32) return mfail(LSPG_EINVAL, "dim must be a multiple of 32 in [32, %d] (got %d)", kMaxDim, dim);
-  if (device < -1) return mfail(LSPG_EINVAL, "device must be >= -1 (got %d)", device);
+  if (dim < 32 || dim > kMaxDim || dim % 32) return fail(LSPG_EINVAL, "dim must be a multiple of 32 in [32, %d] (got %d)", kMaxDim, dim);
+  cudaDeviceProp prop;
+  if (int rc = capi::check_device<Lspm>(device, &prop)) return rc;
   if (device >= 0) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) return mfail(LSPG_ENODEV, "no CUDA device: %s", cudaGetErrorString(e));
-    if (device >= count) return mfail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
-    cudaDeviceProp prop;
-    MCUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0)
-      return mfail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device, prop.major, prop.minor);
     DeviceGuard g(device);
-    MCUDA_TRY(cudaFuncSetAttribute(lspm_knn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(KnnSmem))));
+    CUDA_TRY(cudaFuncSetAttribute(lspm_knn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sizeof(KnnSmem))));
   }
   lspm_ctx* h = new lspm_ctx;
   h->dim = dim;
@@ -416,46 +386,46 @@ int lspm_create(lspm_handle* out, int dim, int device) {
 }
 
 int lspm_load_database(lspm_handle h, const float* host_db, int64_t n_rows) {
-  if (!h || !host_db) return mfail(LSPG_EINVAL, "null argument");
-  if (n_rows < 1 || n_rows >= (static_cast<int64_t>(1) << 31)) return mfail(LSPG_EINVAL, "n_rows must be in [1, 2^31) (got %lld)", static_cast<long long>(n_rows));
-  if (h->device < 0) return mfail(LSPG_ENODEV, "host-only handle: lspm_load_database needs an sm_90 device (no CPU path exists)");
+  if (!h || !host_db) return fail(LSPG_EINVAL, "null argument");
+  if (n_rows < 1 || n_rows >= (static_cast<int64_t>(1) << 31)) return fail(LSPG_EINVAL, "n_rows must be in [1, 2^31) (got %lld)", static_cast<long long>(n_rows));
+  if (int rc = capi::require_device<Lspm>(h->device, "lspm_load_database")) return rc;
   DeviceGuard g(h->device);
   if (n_rows != h->n_rows) {
     if (h->d_db) cudaFree(h->d_db);
     if (h->d_norm) cudaFree(h->d_norm);
     h->d_db = nullptr; h->d_norm = nullptr; h->n_rows = 0;
-    MCUDA_TRY(cudaMalloc(&h->d_db, sizeof(float) * static_cast<size_t>(n_rows) * h->dim));
-    MCUDA_TRY(cudaMalloc(&h->d_norm, sizeof(float) * static_cast<size_t>(n_rows)));
+    CUDA_TRY(cudaMalloc(&h->d_db, sizeof(float) * static_cast<size_t>(n_rows) * h->dim));
+    CUDA_TRY(cudaMalloc(&h->d_norm, sizeof(float) * static_cast<size_t>(n_rows)));
   }
   h->n_rows = 0;                                // not usable until the copy and the norms are complete
-  MCUDA_TRY(cudaMemcpy(h->d_db, host_db, sizeof(float) * static_cast<size_t>(n_rows) * h->dim, cudaMemcpyHostToDevice));
+  CUDA_TRY(cudaMemcpy(h->d_db, host_db, sizeof(float) * static_cast<size_t>(n_rows) * h->dim, cudaMemcpyHostToDevice));
   lspm_norms_kernel<<<ceil_div(static_cast<int>(n_rows), 8), 256>>>(h->d_db, static_cast<int>(n_rows), h->dim, h->d_norm);
-  MCUDA_TRY(cudaGetLastError());
-  MCUDA_TRY(cudaStreamSynchronize(0));
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(0));
   h->n_rows = n_rows;
   return LSPG_OK;
 }
 
 int lspm_workspace_bytes(lspm_handle h, int n, int k, size_t* out) {
-  if (!h || !out) return mfail(LSPG_EINVAL, "null argument");
-  if (n < 1) return mfail(LSPG_EINVAL, "n must be >= 1 (got %d)", n);
-  if (k < 1 || k > kMaxK) return mfail(LSPG_EINVAL, "k must be in [1, %d] (got %d)", kMaxK, k);
+  if (!h || !out) return fail(LSPG_EINVAL, "null argument");
+  if (n < 1) return fail(LSPG_EINVAL, "n must be >= 1 (got %d)", n);
+  if (k < 1 || k > kMaxK) return fail(LSPG_EINVAL, "k must be in [1, %d] (got %d)", kMaxK, k);
   *out = workspace_bytes(n, k);
   return LSPG_OK;
 }
 
 int lspm_knn(lspm_handle h, const float* feats, int n, int k, int64_t* out_ind, float* out_dist_or_null, void* ws,
              size_t ws_bytes, void* stream) {
-  if (!h) return mfail(LSPG_EINVAL, "null handle");
-  if (n < 1) return mfail(LSPG_EINVAL, "n must be >= 1 (got %d)", n);
-  if (k < 1 || k > kMaxK) return mfail(LSPG_EINVAL, "k must be in [1, %d] (got %d)", kMaxK, k);
-  if (h->n_rows > 0 && k > h->n_rows) return mfail(LSPG_EINVAL, "k (%d) exceeds the %lld database rows", k, static_cast<long long>(h->n_rows));
-  if (!feats || !out_ind || !ws) return mfail(LSPG_EINVAL, "null buffer");
-  if (reinterpret_cast<uintptr_t>(feats) % 16) return mfail(LSPG_EINVAL, "feats must be 16-byte aligned");
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (n < 1) return fail(LSPG_EINVAL, "n must be >= 1 (got %d)", n);
+  if (k < 1 || k > kMaxK) return fail(LSPG_EINVAL, "k must be in [1, %d] (got %d)", kMaxK, k);
+  if (h->n_rows > 0 && k > h->n_rows) return fail(LSPG_EINVAL, "k (%d) exceeds the %lld database rows", k, static_cast<long long>(h->n_rows));
+  if (!feats || !out_ind || !ws) return fail(LSPG_EINVAL, "null buffer");
+  if (reinterpret_cast<uintptr_t>(feats) % 16) return fail(LSPG_EINVAL, "feats must be 16-byte aligned");
   const size_t need = workspace_bytes(n, k);
-  if (ws_bytes < need) return mfail(LSPG_EINVAL, "workspace of %zu bytes is smaller than the %zu needed", ws_bytes, need);
-  if (h->device < 0) return mfail(LSPG_ENODEV, "host-only handle: lspm_knn needs an sm_90 device (no CPU path exists)");
-  if (h->n_rows == 0) return mfail(LSPG_ESTATE, "lspm_load_database has not been called");
+  if (ws_bytes < need) return fail(LSPG_EINVAL, "workspace of %zu bytes is smaller than the %zu needed", ws_bytes, need);
+  if (int rc = capi::require_device<Lspm>(h->device, "lspm_knn")) return rc;
+  if (h->n_rows == 0) return fail(LSPG_ESTATE, "lspm_load_database has not been called");
   DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int n_rows = static_cast<int>(h->n_rows);
@@ -472,18 +442,18 @@ int lspm_knn(lspm_handle h, const float* feats, int n, int k, int64_t* out_ind, 
   lspm_knn_kernel<<<dim3(ceil_div(n, kTQ), slices), kKnnThreads, sizeof(KnnSmem), st>>>(
       feats, qn, n, h->d_db, h->d_norm, n_rows, h->dim, k, rows_per_slice, slices, cand_d, cand_i);
   lspm_knn_merge_kernel<<<ceil_div(n, 8), 256, 0, st>>>(cand_d, cand_i, n, slices, k, out_ind, out_dist_or_null);
-  MCUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
 }
 
 int lspm_project(lspm_handle h, const float* feats, int n, const int64_t* ind, int k, float percent, double* out_w,
                  float* out_fuse, float* out_blend, int* out_status, void* stream) {
-  if (!h) return mfail(LSPG_EINVAL, "null handle");
-  if (n < 1) return mfail(LSPG_EINVAL, "n must be >= 1 (got %d)", n);
-  if (k < 1 || k > kMaxK) return mfail(LSPG_EINVAL, "k must be in [1, %d] (got %d)", kMaxK, k);
-  if (!feats || !ind) return mfail(LSPG_EINVAL, "null buffer");
-  if (h->device < 0) return mfail(LSPG_ENODEV, "host-only handle: lspm_project needs an sm_90 device (no CPU path exists)");
-  if (h->n_rows == 0) return mfail(LSPG_ESTATE, "lspm_load_database has not been called");
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (n < 1) return fail(LSPG_EINVAL, "n must be >= 1 (got %d)", n);
+  if (k < 1 || k > kMaxK) return fail(LSPG_EINVAL, "k must be in [1, %d] (got %d)", kMaxK, k);
+  if (!feats || !ind) return fail(LSPG_EINVAL, "null buffer");
+  if (int rc = capi::require_device<Lspm>(h->device, "lspm_project")) return rc;
+  if (h->n_rows == 0) return fail(LSPG_ESTATE, "lspm_load_database has not been called");
   DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   // demo.py:200 multiplies the float32 features by the Python float (1 - LLE_percent): that product is formed in
@@ -497,7 +467,7 @@ int lspm_project(lspm_handle h, const float* feats, int n, const int64_t* ind, i
     lspm_lle_kernel<7><<<grid, block, 0, st>>>(feats, n, h->d_db, h->n_rows, h->dim, ind, k, percent, omp, out_w, out_fuse, out_blend, out_status);
   else
     lspm_lle_kernel<17><<<grid, block, 0, st>>>(feats, n, h->d_db, h->n_rows, h->dim, ind, k, percent, omp, out_w, out_fuse, out_blend, out_status);
-  MCUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
 }
 

@@ -21,38 +21,22 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
-#include <cstdio>
 #include <cstring>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
 
 #include "../../include/lspr.h"
+#include "capi.cuh"
 #include "gemm_nt.cuh"
 
 namespace cg = cooperative_groups;
+using capi::DeviceGuard;
 
 namespace {
 
-thread_local std::string g_rerr;
-
-int rfail(int code, const char* fmt, ...) {
-  char buf[1024];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  g_rerr = buf;
-  return code;
-}
-
-#define RCUDA_TRY(expr)                                                                           \
-  do {                                                                                            \
-    cudaError_t _e = (expr);                                                                      \
-    if (_e != cudaSuccess) return rfail(LSPG_ECUDA, "%s failed: %s", #expr, cudaGetErrorString(_e)); \
-  } while (0)
+struct Lspr;
+constexpr auto fail = capi::fail<Lspr>;
 
 constexpr int kNW = 16;            // warps per CTA of the recurrence
 constexpr int kApcH = 512;         // APC hidden size the GRU kernels are built for
@@ -213,13 +197,13 @@ int launch_rnn(lspr_ctx* h, int cl, const RecParams& p, cudaStream_t st) {
   cfg.attrs = attr; cfg.numAttrs = 1;
   if (h->G == 4) {
     cfg.dynamicSmemBytes = kLstm8Smem;
-    RCUDA_TRY(cudaLaunchKernelEx(&cfg, LSTM8, p));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, LSTM8, p));
   } else if (cl == 16) {
     cfg.dynamicSmemBytes = kGru16Smem;
-    RCUDA_TRY(cudaLaunchKernelEx(&cfg, GRU16, p));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, GRU16, p));
   } else {
     cfg.dynamicSmemBytes = kGru8Smem;
-    RCUDA_TRY(cudaLaunchKernelEx(&cfg, GRU8, p));
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, GRU8, p));
   }
   return LSPG_OK;
 }
@@ -234,8 +218,8 @@ int max_clusters(K kernel, int cl, size_t smem, int* out) {
   attr[0].id = cudaLaunchAttributeClusterDimension;
   attr[0].val.clusterDim.x = cl; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
-  RCUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-  if (cl > 8) RCUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
+  CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  if (cl > 8) CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
   *out = 0;
   if (cudaOccupancyMaxActiveClusters(out, kernel, &cfg) != cudaSuccess) {
     cudaGetLastError();              // "cannot be scheduled" comes back as an error on some drivers: treat it as 0
@@ -253,38 +237,33 @@ void gemm(const float* A, const float* W, const float* scale, const float* shift
 
 extern "C" {
 
-const char* lspr_last_error(void) { return g_rerr.c_str(); }
+const char* lspr_last_error(void) { return capi::last_error<Lspr>().c_str(); }
 
 int lspr_create(lspr_handle* out, const lspr_config* c, int device) {
-  if (!out || !c) return rfail(LSPG_EINVAL, "null argument");
+  if (!out || !c) return fail(LSPG_EINVAL, "null argument");
   *out = nullptr;
   std::unique_ptr<lspr_ctx> h(new lspr_ctx);
   h->cfg = *c;
   h->device = device;
   if (c->kind == LSPR_APC) {
-    if (c->hidden != kApcH) return rfail(LSPG_EINVAL, "APC hidden_size must be %d (got %d)", kApcH, c->hidden);
-    if (c->input_dim < 16 || c->input_dim % 16) return rfail(LSPG_EINVAL, "APC mel_dim must be a positive multiple of 16 (got %d)", c->input_dim);
-    if (c->num_layers < 1 || c->num_layers > kMaxApcLayers) return rfail(LSPG_EINVAL, "APC num_layers must be in [1, %d] (got %d)", kMaxApcLayers, c->num_layers);
+    if (c->hidden != kApcH) return fail(LSPG_EINVAL, "APC hidden_size must be %d (got %d)", kApcH, c->hidden);
+    if (c->input_dim < 16 || c->input_dim % 16) return fail(LSPG_EINVAL, "APC mel_dim must be a positive multiple of 16 (got %d)", c->input_dim);
+    if (c->num_layers < 1 || c->num_layers > kMaxApcLayers) return fail(LSPG_EINVAL, "APC num_layers must be in [1, %d] (got %d)", kMaxApcLayers, c->num_layers);
     h->G = 3; h->H = kApcH; h->L = c->num_layers;
     for (int l = 0; l < h->L; ++l) h->in_w.push_back(l == 0 ? c->input_dim : kApcH);
   } else if (c->kind == LSPR_MOUTH) {
-    if (c->input_dim < 64 || c->input_dim % 64) return rfail(LSPG_EINVAL, "APC_hidden_size must be a positive multiple of 64 (got %d)", c->input_dim);
-    if (c->frame_future < 0) return rfail(LSPG_EINVAL, "frame_future must be >= 0 (got %d)", c->frame_future);
-    if (c->out_dim < 1 || c->out_dim > kMaxOut) return rfail(LSPG_EINVAL, "out_dim must be in [1, %d] (got %d)", kMaxOut, c->out_dim);
+    if (c->input_dim < 64 || c->input_dim % 64) return fail(LSPG_EINVAL, "APC_hidden_size must be a positive multiple of 64 (got %d)", c->input_dim);
+    if (c->frame_future < 0) return fail(LSPG_EINVAL, "frame_future must be >= 0 (got %d)", c->frame_future);
+    if (c->out_dim < 1 || c->out_dim > kMaxOut) return fail(LSPG_EINVAL, "out_dim must be in [1, %d] (got %d)", kMaxOut, c->out_dim);
     h->G = 4; h->H = kLstmH; h->L = 3;
     for (int l = 0; l < h->L; ++l) h->in_w.push_back(l == 0 ? c->input_dim : kLstmH);
   } else {
-    return rfail(LSPG_EINVAL, "kind must be LSPR_APC or LSPR_MOUTH (got %d)", c->kind);
+    return fail(LSPG_EINVAL, "kind must be LSPR_APC or LSPR_MOUTH (got %d)", c->kind);
   }
+  cudaDeviceProp prop;
+  if (int rc = capi::check_device<Lspr>(device, &prop)) return rc;
   if (device >= 0) {
-    int count = 0;
-    cudaError_t e = cudaGetDeviceCount(&count);
-    if (e != cudaSuccess || count == 0) return rfail(LSPG_ENODEV, "no CUDA device: %s", cudaGetErrorString(e));
-    if (device >= count) return rfail(LSPG_ENODEV, "device %d out of range (%d devices)", device, count);
-    cudaDeviceProp prop;
-    RCUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 9 || prop.minor != 0) return rfail(LSPG_ENODEV, "device %d is sm_%d%d; this library contains sm_90a code only (no fallback)", device, prop.major, prop.minor);
-    RCUDA_TRY(cudaSetDevice(device));
+    DeviceGuard g(device);
     int r;
     if (h->G == 3) {
       if ((r = max_clusters(GRU16, 16, kGru16Smem, &h->max_clusters16))) return r;
@@ -300,7 +279,7 @@ int lspr_create(lspr_handle* out, const lspr_config* c, int device) {
 int lspr_destroy(lspr_handle h) {
   if (!h) return LSPG_OK;
   if (h->device >= 0) {
-    cudaSetDevice(h->device);
+    DeviceGuard g(h->device);
     for (float* p : h->d_packed) if (p) cudaFree(p);
     if (h->d_ones) cudaFree(h->d_ones);
   }
@@ -309,28 +288,10 @@ int lspr_destroy(lspr_handle h) {
 }
 
 int lspr_load_weights(lspr_handle h, const lspg_tensor* tensors, int n) {
-  if (!h || (!tensors && n > 0)) return rfail(LSPG_EINVAL, "null argument");
+  if (!h || (!tensors && n > 0)) return fail(LSPG_EINVAL, "null argument");
   const lspr_config& c = h->cfg;
-  std::map<std::string, const lspg_tensor*> by_name;
-  for (int i = 0; i < n; ++i) {
-    if (!tensors[i].name || !tensors[i].data) return rfail(LSPG_EINVAL, "tensor %d has a null name or data pointer", i);
-    std::string nm = tensors[i].name;
-    if (nm.rfind("module.", 0) == 0) nm = nm.substr(7);
-    by_name[nm] = &tensors[i];
-  }
-  int rc = LSPG_OK;
-  auto get = [&](const std::string& key, size_t expect) -> const float* {
-    auto it = by_name.find(key);
-    if (it == by_name.end()) {
-      if (rc == LSPG_OK) rc = rfail(LSPG_ESTATE, "missing parameter %s", key.c_str());
-      return nullptr;
-    }
-    if (static_cast<size_t>(it->second->numel) != expect) {
-      if (rc == LSPG_OK) rc = rfail(LSPG_EINVAL, "%s has %lld elements, expected %zu", key.c_str(), static_cast<long long>(it->second->numel), expect);
-      return nullptr;
-    }
-    return it->second->data;
-  };
+  capi::WeightTable<Lspr> wt(tensors, n);
+  if (int rc = wt.status()) return rc;
   const int G = h->G, H = h->H;
   std::vector<std::vector<float>> packed;
   // ---- recurrent layers: gate rows interleaved by unit, biases folded except the GRU's b_hn
@@ -338,11 +299,11 @@ int lspr_load_weights(lspr_handle h, const lspg_tensor* tensors, int n) {
     const int In = h->in_w[l];
     const std::string p = c.kind == LSPR_APC ? "rnns." + std::to_string(l) + "." : "LSTM.";
     const std::string sfx = c.kind == LSPR_APC ? "_l0" : "_l" + std::to_string(l);
-    const float* wih = get(p + "weight_ih" + sfx, static_cast<size_t>(G) * H * In);
-    const float* whh = get(p + "weight_hh" + sfx, static_cast<size_t>(G) * H * H);
-    const float* bih = get(p + "bias_ih" + sfx, static_cast<size_t>(G) * H);
-    const float* bhh = get(p + "bias_hh" + sfx, static_cast<size_t>(G) * H);
-    if (rc) return rc;
+    const float* wih = wt.get(p + "weight_ih" + sfx, static_cast<size_t>(G) * H * In);
+    const float* whh = wt.get(p + "weight_hh" + sfx, static_cast<size_t>(G) * H * H);
+    const float* bih = wt.get(p + "bias_ih" + sfx, static_cast<size_t>(G) * H);
+    const float* bhh = wt.get(p + "bias_hh" + sfx, static_cast<size_t>(G) * H);
+    if (int rc = wt.status()) return rc;
     std::vector<float> w_ih(static_cast<size_t>(G) * H * In), b(static_cast<size_t>(G) * H), w_hh(static_cast<size_t>(G) * H * H);
     std::vector<float> b_hn(G == 3 ? H : 0);
     for (int u = 0; u < H; ++u)
@@ -366,15 +327,15 @@ int lspr_load_weights(lspr_handle h, const lspg_tensor* tensors, int n) {
                              {"fc.0", "fc.1", kFcW, kLstmH}, {"fc.3", "fc.4", kFcW, kFcW}, {"fc.6", nullptr, c.out_dim, kFcW}};
     for (const Stage& s : stages) {
       const std::string lin = s.lin;
-      const float* w = get(lin + ".weight", static_cast<size_t>(s.n) * s.k);
-      const float* bias = get(lin + ".bias", s.n);
+      const float* w = wt.get(lin + ".weight", static_cast<size_t>(s.n) * s.k);
+      const float* bias = wt.get(lin + ".bias", s.n);
       const float *bw = nullptr, *bb = nullptr, *bm = nullptr, *bv = nullptr;
       if (s.bn) {
         const std::string bn = s.bn;
-        bw = get(bn + ".weight", s.n); bb = get(bn + ".bias", s.n);
-        bm = get(bn + ".running_mean", s.n); bv = get(bn + ".running_var", s.n);
+        bw = wt.get(bn + ".weight", s.n); bb = wt.get(bn + ".bias", s.n);
+        bm = wt.get(bn + ".running_mean", s.n); bv = wt.get(bn + ".running_var", s.n);
       }
-      if (rc) return rc;
+      if (int rc = wt.status()) return rc;
       std::vector<float> scale(s.n, 1.0f), shift(bias, bias + s.n);
       if (s.bn)
         for (int j = 0; j < s.n; ++j) {
@@ -388,23 +349,23 @@ int lspr_load_weights(lspr_handle h, const lspg_tensor* tensors, int n) {
     }
   }
   if (h->device >= 0) {
-    RCUDA_TRY(cudaSetDevice(h->device));
-    RCUDA_TRY(cudaDeviceSynchronize());          // no launch still reads the arrays being replaced
+    DeviceGuard g(h->device);
+    CUDA_TRY(cudaDeviceSynchronize());          // no launch still reads the arrays being replaced
     if (h->d_packed.size() != packed.size()) h->d_packed.assign(packed.size(), nullptr);
     for (size_t i = 0; i < packed.size(); ++i) {
       if (h->d_packed[i] && (h->packed.size() != packed.size() || h->packed[i].size() != packed[i].size())) {
         cudaFree(h->d_packed[i]);
         h->d_packed[i] = nullptr;
       }
-      if (!h->d_packed[i] && !packed[i].empty()) RCUDA_TRY(cudaMalloc(&h->d_packed[i], sizeof(float) * packed[i].size()));
+      if (!h->d_packed[i] && !packed[i].empty()) CUDA_TRY(cudaMalloc(&h->d_packed[i], sizeof(float) * packed[i].size()));
       if (!packed[i].empty())
-        RCUDA_TRY(cudaMemcpy(h->d_packed[i], packed[i].data(), sizeof(float) * packed[i].size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(h->d_packed[i], packed[i].data(), sizeof(float) * packed[i].size(), cudaMemcpyHostToDevice));
     }
     if (!h->d_ones) {
       h->n_ones = static_cast<size_t>(G) * H;
       std::vector<float> ones(h->n_ones, 1.0f);
-      RCUDA_TRY(cudaMalloc(&h->d_ones, sizeof(float) * h->n_ones));
-      RCUDA_TRY(cudaMemcpy(h->d_ones, ones.data(), sizeof(float) * h->n_ones, cudaMemcpyHostToDevice));
+      CUDA_TRY(cudaMalloc(&h->d_ones, sizeof(float) * h->n_ones));
+      CUDA_TRY(cudaMemcpy(h->d_ones, ones.data(), sizeof(float) * h->n_ones, cudaMemcpyHostToDevice));
     }
   }
   h->packed = std::move(packed);
@@ -413,13 +374,13 @@ int lspr_load_weights(lspr_handle h, const lspg_tensor* tensors, int n) {
 }
 
 int lspr_debug_packed(lspr_handle h, int which, float* dst, int64_t* count) {
-  if (!h || !count) return rfail(LSPG_EINVAL, "null argument");
-  if (!h->weights_loaded) return rfail(LSPG_ESTATE, "weights not loaded");
+  if (!h || !count) return fail(LSPG_EINVAL, "null argument");
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "weights not loaded");
   if (which < 0 || which >= static_cast<int>(h->packed.size()))
-    return rfail(LSPG_EINVAL, "which must be in [0, %zu) (got %d)", h->packed.size(), which);
+    return fail(LSPG_EINVAL, "which must be in [0, %zu) (got %d)", h->packed.size(), which);
   const std::vector<float>& v = h->packed[which];
   if (!dst) { *count = static_cast<int64_t>(v.size()); return LSPG_OK; }
-  if (static_cast<size_t>(*count) != v.size()) return rfail(LSPG_EINVAL, "count %lld != %zu", static_cast<long long>(*count), v.size());
+  if (static_cast<size_t>(*count) != v.size()) return fail(LSPG_EINVAL, "count %lld != %zu", static_cast<long long>(*count), v.size());
   if (!v.empty()) memcpy(dst, v.data(), sizeof(float) * v.size());
   return LSPG_OK;
 }
@@ -443,41 +404,41 @@ static size_t workspace_floats(const lspr_ctx* h, int n_rows, size_t off[5]) {
 }
 
 int lspr_workspace_bytes(lspr_handle h, int n_rows, size_t* bytes) {
-  if (!h || !bytes) return rfail(LSPG_EINVAL, "null argument");
-  if (n_rows < 0) return rfail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
+  if (!h || !bytes) return fail(LSPG_EINVAL, "null argument");
+  if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
   size_t off[5];
   *bytes = sizeof(float) * workspace_floats(h, n_rows, off);
   return LSPG_OK;
 }
 
 int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* ws, size_t ws_bytes, int cluster, void* stream) {
-  if (!h) return rfail(LSPG_EINVAL, "null handle");
-  if (h->device < 0) return rfail(LSPG_ENODEV, "host-only handle: lspr_forward needs an sm_90 device (no CPU path exists)");
-  if (!h->weights_loaded) return rfail(LSPG_ESTATE, "lspr_load_weights has not been called");
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (int rc = capi::require_device<Lspr>(h->device, "lspr_forward")) return rc;
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
   const lspr_config& c = h->cfg;
   const bool apc = c.kind == LSPR_APC;
-  if (n_rows < 0) return rfail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
+  if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
   if (!apc && (n_rows < 2 || n_rows % 2))
-    return rfail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even and >= 2 (got %d)", n_rows);
-  if (n_rows > 0 && (!in || !out)) return rfail(LSPG_EINVAL, "null buffer");
-  if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) % 16) return rfail(LSPG_EINVAL, "in and out must be 16-byte aligned");
+    return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even and >= 2 (got %d)", n_rows);
+  if (n_rows > 0 && (!in || !out)) return fail(LSPG_EINVAL, "null buffer");
+  if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) % 16) return fail(LSPG_EINVAL, "in and out must be 16-byte aligned");
   size_t off[5];
   const size_t need = sizeof(float) * workspace_floats(h, n_rows, off);
-  if (ws_bytes < need) return rfail(LSPG_EINVAL, "workspace of %zu bytes is smaller than the %zu needed", ws_bytes, need);
-  if (need && (!ws || reinterpret_cast<uintptr_t>(ws) % 256)) return rfail(LSPG_EINVAL, "workspace must be non-null and 256-byte aligned");
+  if (ws_bytes < need) return fail(LSPG_EINVAL, "workspace of %zu bytes is smaller than the %zu needed", ws_bytes, need);
+  if (need && (!ws || reinterpret_cast<uintptr_t>(ws) % 256)) return fail(LSPG_EINVAL, "workspace must be non-null and 256-byte aligned");
   int cl = cluster;
   if (apc) {
     if (cl == 0) cl = h->max_clusters16 > 0 ? 16 : 8;
-    if (cl != 8 && cl != 16) return rfail(LSPG_EINVAL, "APC cluster must be 0, 8 or 16 (got %d)", cluster);
+    if (cl != 8 && cl != 16) return fail(LSPG_EINVAL, "APC cluster must be 0, 8 or 16 (got %d)", cluster);
   } else {
     if (cl == 0) cl = 8;
-    if (cl != 8) return rfail(LSPG_EINVAL, "Audio2Mouth cluster must be 0 or 8 (got %d)", cluster);
+    if (cl != 8) return fail(LSPG_EINVAL, "Audio2Mouth cluster must be 0 or 8 (got %d)", cluster);
   }
   if ((cl == 16 ? h->max_clusters16 : h->max_clusters8) < 1)
-    return rfail(LSPG_ENODEV, "a %d-CTA cluster with %zu bytes of shared memory per CTA cannot be scheduled on device %d", cl,
+    return fail(LSPG_ENODEV, "a %d-CTA cluster with %zu bytes of shared memory per CTA cannot be scheduled on device %d", cl,
                  cl == 16 ? kGru16Smem : (apc ? kGru8Smem : kLstm8Smem), h->device);
   if (n_rows == 0) return LSPG_OK;
-  RCUDA_TRY(cudaSetDevice(h->device));
+  DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* w = static_cast<float*>(ws);
   const int G = h->G, H = h->H;
@@ -516,7 +477,7 @@ int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* w
     gemm_nt_kernel<true, false><<<dim3((c.out_dim + 63) / 64, (nframe + 63) / 64), 256, 0, st>>>(m1, P(24), P(25), P(26), out,
                                                                                                nframe, c.out_dim, kFcW, 0, 0);
   }
-  RCUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
 }
 

@@ -157,9 +157,7 @@ class Feature2Face_G(nn.Module):
             "livespeechportraits_b200.parallel.ShardedRenderer")
 
     def _ensure_handle(self, device: torch.device) -> None:
-        if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: inputs must live on an H100 (sm_90) device")
-        idx = device.index if device.index is not None else torch.cuda.current_device()
+        idx = _lib.cuda_device(device, "the generator's input").index
         if self._handle and self._device_index == idx:
             return
         if self._handle:
@@ -174,20 +172,8 @@ class Feature2Face_G(nn.Module):
         self._workspaces.clear()
 
     def _push_weights(self) -> None:
-        sd = super().state_dict()
-        names: List[bytes] = []
-        keep: List[torch.Tensor] = []
-        for k, v in sd.items():
-            if k.endswith("num_batches_tracked"):
-                continue
-            names.append(k.encode())
-            keep.append(v.detach().to(device="cpu", dtype=torch.float32).contiguous())
-        arr = (_lib.LspgTensor * len(keep))()
-        for i, (nm, t) in enumerate(zip(names, keep)):
-            arr[i].name = nm
-            arr[i].data = C.cast(t.data_ptr(), C.POINTER(C.c_float))
-            arr[i].numel = t.numel()
-        _lib.check(self._lib.lspg_load_weights(self._handle, arr, len(keep)))
+        arr, _keep = _lib.tensor_array(super().state_dict())
+        _lib.check(self._lib.lspg_load_weights(self._handle, arr, len(arr)))
         self._weights_dirty = False
 
     # ------------------------------------------------------------------ forward

@@ -47,40 +47,24 @@ def config_from_opt(opt) -> _lib.LsphConfig:
     return cfg
 
 
-class HeadposeGenerator:
+class HeadposeGenerator(_lib.Handle):
     """Owns the native handle (packed weights on one device).  ``state_dict`` uses the key grammar of
     ``Audio2Headpose(opt).state_dict()`` (an optional ``module.`` prefix is accepted)."""
+    prefix, what = "lsph", "the headpose loop"
 
     def __init__(self, opt, state_dict: Dict[str, torch.Tensor], device: Optional[torch.device] = None):
-        self._lib = _lib.load()
-        self._handle = C.c_void_p()
         self.cfg = config_from_opt(opt)
-        if device is None:
-            device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: the headpose loop needs an H100 (sm_90) device")
-        self.device = device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
-        _lib.check_h(self._lib.lsph_create(C.byref(self._handle), C.byref(self.cfg), self.device.index))
+        super().__init__(device)
+        self._create(C.byref(self.cfg))
         rf = C.c_int()
-        _lib.check_h(self._lib.lsph_receptive_field(self._handle, C.byref(rf)))
+        self.call("receptive_field", C.byref(rf))
         self.receptive_field = rf.value
         self.out_channels = (2 * self.cfg.ndim + 1) * self.cfg.ncenter if self.cfg.loss_gmm else self.cfg.ndim
         self.load_state_dict(state_dict)
 
     def load_state_dict(self, state_dict: Dict[str, torch.Tensor]) -> None:
-        names, keep = [], []
-        for k, v in state_dict.items():
-            if k.endswith("num_batches_tracked"):
-                continue
-            names.append(k.encode())
-            keep.append(v.detach().to(device="cpu", dtype=torch.float32).contiguous())
-        arr = (_lib.LspgTensor * len(keep))()
-        for i, (nm, t) in enumerate(zip(names, keep)):
-            arr[i].name = nm
-            arr[i].data = C.cast(t.data_ptr(), C.POINTER(C.c_float))
-            arr[i].numel = t.numel()
-        _lib.check_h(self._lib.lsph_load_weights(self._handle, arr, len(keep)))
+        arr, _keep = _lib.tensor_array(state_dict)
+        self.call("load_weights", arr, len(arr))
 
     def generate(self, audio_feats, pre_headpose, noise, sigma_scale: float, uniform=None, return_params: bool = False,
                  cluster: int = 0):
@@ -104,21 +88,12 @@ class HeadposeGenerator:
         for t in (a, pre, nz):
             if t.data_ptr() % 16:
                 raise ValueError("device buffers must be 16-byte aligned")
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check_h(self._lib.lsph_generate(self._handle, a.data_ptr(), n_audio, pre.data_ptr(), nz.data_ptr(),
-                                                 un.data_ptr() if un is not None else None, float(sigma_scale), pred.data_ptr(),
-                                                 params.data_ptr() if params is not None else None, int(cluster), stream))
+        with self.stream() as stream:
+            self.call("generate", a.data_ptr(), n_audio, pre.data_ptr(), nz.data_ptr(), un.data_ptr() if un is not None else None,
+                      float(sigma_scale), pred.data_ptr(), params.data_ptr() if params is not None else None, int(cluster),
+                      stream)
         self._keep = (a, pre, nz, un)            # inputs stay alive until the caller synchronises on the result
         return (pred, params) if return_params else pred
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.lsph_destroy(self._handle)
-                self._handle = C.c_void_p()
-        except Exception:
-            pass
 
 
 def draw_reference_noise(nframe: int, ndim: int, ncenter: int):
@@ -145,20 +120,7 @@ def generate_sequences(self, audio_feats, pre_headpose, fill_zero=True, sigma_sc
     if not fill_zero:
         return None                                                                    # audio2headpose_model.py:161-162
     net = self.Audio2Headpose.module if hasattr(self.Audio2Headpose, "module") else self.Audio2Headpose
-    sd = net.state_dict()
-    # the packed copy on the device is reused while the module's tensors are untouched: tensor version counters move on every
-    # in-place write (load_state_dict copies in place, optimiser steps, init_weights), data pointers on re-allocation (.to())
-    stamp = tuple((v.data_ptr(), v._version) for v in sd.values())
-    hit = _GENERATORS.get(id(net))
-    if hit is None or hit[1] != stamp:
-        if hit is None:
-            gen = HeadposeGenerator(opt, sd)
-        else:
-            gen = hit[0]
-            gen.load_state_dict(sd)
-        _GENERATORS.clear()
-        _GENERATORS[id(net)] = (gen, stamp)
-    gen = _GENERATORS[id(net)][0]
+    gen = _lib.cached(_GENERATORS, net, lambda sd: HeadposeGenerator(opt, sd))
     audio = np.asarray(audio_feats, dtype=np.float32).reshape(-1, 512 * 2)              # :148
     nframe = audio.shape[0] - opt.frame_future
     if getattr(opt, "loss", "GMM") == "GMM":

@@ -111,18 +111,12 @@ def _native_params(p: StageParams, image_pad) -> _lib.LsplParams:
     return n
 
 
-class LandmarkPostprocessor:
+class LandmarkPostprocessor(_lib.Handle):
     """Owns the native handle and the device copy of one identity's constants (taken at construction)."""
+    prefix, what = "lspl", "the landmark post-processing"
 
     def __init__(self, identity: Identity, device: Optional[torch.device] = None):
-        self._lib = _lib.load()
-        self._handle = C.c_void_p()
-        if device is None:
-            device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: the landmark post-processing needs an H100 (sm_90) device")
-        self.device = device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
+        super().__init__(device)
         cand = np.ascontiguousarray(np.asarray(identity.candidate_eye_brow, dtype=np.float64))
         if cand.ndim != 3 or cand.shape[1:] != (16, 3) or cand.shape[0] < 1:
             raise ValueError(f"candidate_eye_brow must be [m >= 1, 16, 3], got {cand.shape}")
@@ -139,8 +133,8 @@ class LandmarkPostprocessor:
         nid.relative_rotation[:] = _f64(rv, (3, 3)).ravel().tolist()
         nid.relative_translation[:] = _f64(tv, (3,)).tolist()
         nid.scale = float(identity.scale)
-        _lib.check_l(self._lib.lspl_create(C.byref(self._handle), self.device.index))
-        _lib.check_l(self._lib.lspl_load_identity(self._handle, C.byref(nid)))
+        self._create()
+        self.call("load_identity", C.byref(nid))
         del self._keep
 
     def run(self, pred_feat, pred_head, params: StageParams, image_pad: Optional[Sequence[int]] = None,
@@ -169,23 +163,12 @@ class LandmarkPostprocessor:
         sh = torch.empty((n, N_SHOULDERS, 2), **f32)
         pts = torch.empty((n, N_PTS, 3), **f32) if return_intermediates else None
         pose = torch.empty((n, 6), **f32) if return_intermediates else None
-        nbytes = C.c_size_t()
-        _lib.check_l(self._lib.lspl_workspace_bytes(self._handle, n_feat, n_head, C.byref(nbytes)))
-        ws = torch.empty((max(nbytes.value, 1),), dtype=torch.uint8, device=dev)
+        ws = self.workspace(n_feat, n_head)
         ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None    # noqa: E731
-        with torch.cuda.device(dev):
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            _lib.check_l(self._lib.lspl_run(self._handle, ptr(feat), n_feat, ptr(head), n_head, head.shape[1], C.byref(native),
-                                            ptr(lm), ptr(sh), ptr(pts), ptr(pose), ws.data_ptr(), ws.numel(), stream))
+        with self.stream() as stream:
+            self.call("run", ptr(feat), n_feat, ptr(head), n_head, head.shape[1], C.byref(native), ptr(lm), ptr(sh), ptr(pts),
+                      ptr(pose), ws.data_ptr(), ws.numel(), stream)
         return (lm, sh, pts, pose) if return_intermediates else (lm, sh)
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.lspl_destroy(self._handle)
-                self._handle = C.c_void_p()
-        except Exception:
-            pass
 
 
 def postprocess_clip(pred_Feat, pred_Head, mean_pts3d, std_mean_pts3d, candidate_eye_brow, mean_translation, ref_trans,

@@ -12,7 +12,6 @@ attributes, so it then runs unchanged.  There is no CPU path.
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Optional, Tuple
 
 import numpy as np
@@ -24,27 +23,21 @@ MAX_K = 32
 STATUS_OK, STATUS_SINGULAR, STATUS_BAD_INDEX = 0, 1, 2
 
 
-class ManifoldProjector:
+class ManifoldProjector(_lib.Handle):
     """Owns the native handle and the device copy of one feature base ``database`` [N, dim] (fp32; dim a multiple of 32,
     at most 1024).  The copy is taken at construction: later edits to the caller's array are not seen."""
+    prefix, what = "lspm", "the manifold projection"
 
     def __init__(self, database, device: Optional[torch.device] = None):
-        self._lib = _lib.load()
-        self._handle = C.c_void_p()
-        if device is None:
-            device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-        device = torch.device(device)
-        if device.type != "cuda":
-            raise RuntimeError("livespeechportraits_b200 has no CPU path: the manifold projection needs an H100 (sm_90) device")
-        self.device = device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
+        super().__init__(device)
         if isinstance(database, torch.Tensor):
             database = database.detach().cpu().numpy()
         db = np.ascontiguousarray(database, dtype=np.float32)
         if db.ndim != 2:
             raise ValueError(f"database must be [N, dim], got shape {db.shape}")
         self.n_rows, self.dim = db.shape
-        _lib.check_m(self._lib.lspm_create(C.byref(self._handle), int(self.dim), self.device.index))
-        _lib.check_m(self._lib.lspm_load_database(self._handle, db.ctypes.data, int(self.n_rows)))
+        self._create(int(self.dim))
+        self.call("load_database", db.ctypes.data, int(self.n_rows))
 
     def _feats(self, feats) -> torch.Tensor:
         f = torch.as_tensor(feats).to(device=self.device, dtype=torch.float32).contiguous()
@@ -64,14 +57,10 @@ class ManifoldProjector:
         k = int(k)
         if not 1 <= k <= min(MAX_K, self.n_rows):
             raise ValueError(f"k must be in [1, {min(MAX_K, self.n_rows)}] (got {k})")
-        need = C.c_size_t()
-        _lib.check_m(self._lib.lspm_workspace_bytes(self._handle, n, k, C.byref(need)))
-        ws = torch.empty(max(1, need.value), dtype=torch.uint8, device=self.device)
+        ws = self.workspace(n, k)
         ind = torch.empty((n, k), dtype=torch.int64, device=self.device)
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            _lib.check_m(self._lib.lspm_knn(self._handle, f.data_ptr(), n, k, ind.data_ptr(), None, ws.data_ptr(),
-                                            need.value, stream))
+        with self.stream() as stream:
+            self.call("knn", f.data_ptr(), n, k, ind.data_ptr(), None, ws.data_ptr(), ws.numel(), stream)
         return ind
 
     def project(self, feats, ind, percent: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -90,10 +79,9 @@ class ManifoldProjector:
         fuse = torch.empty((n, self.dim), dtype=torch.float32, device=self.device)
         blend = torch.empty((n, self.dim), dtype=torch.float32, device=self.device)
         status = torch.empty((n,), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            _lib.check_m(self._lib.lspm_project(self._handle, f.data_ptr(), n, ix.data_ptr(), k, float(percent), w.data_ptr(),
-                                                fuse.data_ptr(), blend.data_ptr(), status.data_ptr(), stream))
+        with self.stream() as stream:
+            self.call("project", f.data_ptr(), n, ix.data_ptr(), k, float(percent), w.data_ptr(), fuse.data_ptr(),
+                      blend.data_ptr(), status.data_ptr(), stream)
         return w, fuse, blend, status
 
     def project_features(self, feats, k: int, percent: float = 1.0) -> torch.Tensor:
@@ -102,14 +90,6 @@ class ManifoldProjector:
         f = self._feats(feats)
         ind = self.knn(f, k)
         return self.project(f, ind, percent)[2]
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.lspm_destroy(self._handle)
-                self._handle = C.c_void_p()
-        except Exception:
-            pass
 
 
 def _float32_array(name: str, a) -> np.ndarray:

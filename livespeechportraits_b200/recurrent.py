@@ -24,46 +24,26 @@ from . import _lib
 LSTM_HIDDEN = 256          # models/audio2feature.py:40
 
 
-def _cuda_device(device) -> torch.device:
-    if device is None:
-        device = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() else torch.device("cpu")
-    device = torch.device(device)
-    if device.type != "cuda":
-        raise RuntimeError("livespeechportraits_b200 has no CPU path: the recurrent networks need an H100 (sm_90) device")
-    return device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
-
-
-class _Recurrent:
+class _Recurrent(_lib.Handle):
     """Owns one native handle (packed weights on one device)."""
+    prefix = "lspr"
 
     def __init__(self, cfg: _lib.LsprConfig, state_dict: Dict[str, torch.Tensor], device):
-        self._lib = _lib.load()
-        self._handle = C.c_void_p()
+        super().__init__(device)
         self.cfg = cfg
-        self.device = _cuda_device(device) if device != -1 else None
-        _lib.check_r(self._lib.lspr_create(C.byref(self._handle), C.byref(cfg), self.device.index if self.device else -1))
+        self._create(C.byref(cfg))
         self.load_state_dict(state_dict)
 
     def load_state_dict(self, state_dict: Dict[str, torch.Tensor]) -> None:
-        names, keep = [], []
-        for k, v in state_dict.items():
-            if k.endswith("num_batches_tracked"):
-                continue
-            names.append(k.encode())
-            keep.append(v.detach().to(device="cpu", dtype=torch.float32).contiguous())
-        arr = (_lib.LspgTensor * len(keep))()
-        for i, (nm, t) in enumerate(zip(names, keep)):
-            arr[i].name = nm
-            arr[i].data = C.cast(t.data_ptr(), C.POINTER(C.c_float))
-            arr[i].numel = t.numel()
-        _lib.check_r(self._lib.lspr_load_weights(self._handle, arr, len(keep)))
+        arr, _keep = _lib.tensor_array(state_dict)
+        self.call("load_weights", arr, len(arr))
 
     def packed(self, which: int) -> np.ndarray:
         """The array ``lspr_debug_packed`` returns (see include/lspr.h for the order)."""
         n = C.c_int64()
-        _lib.check_r(self._lib.lspr_debug_packed(self._handle, which, None, C.byref(n)))
+        self.call("debug_packed", which, None, C.byref(n))
         out = np.empty(n.value, np.float32)
-        _lib.check_r(self._lib.lspr_debug_packed(self._handle, which, out.ctypes.data, C.byref(n)))
+        self.call("debug_packed", which, out.ctypes.data, C.byref(n))
         return out
 
     def _run(self, x: torch.Tensor, width: int, out_shape, cluster: int) -> torch.Tensor:
@@ -78,29 +58,18 @@ class _Recurrent:
             x = x.clone()
         n = x.shape[0]
         out = torch.empty(out_shape, dtype=torch.float32, device=self.device)
-        nbytes = C.c_size_t()
-        _lib.check_r(self._lib.lspr_workspace_bytes(self._handle, n, C.byref(nbytes)))
-        ws = torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=self.device)
-        with torch.cuda.device(self.device):
-            stream = torch.cuda.current_stream(self.device).cuda_stream
-            _lib.check_r(self._lib.lspr_forward(self._handle, x.data_ptr(), n, out.data_ptr(), ws.data_ptr(), nbytes.value,
-                                                int(cluster), stream))
+        ws = self.workspace(n)
+        with self.stream() as stream:
+            self.call("forward", x.data_ptr(), n, out.data_ptr(), ws.data_ptr(), ws.numel(), int(cluster), stream)
         self._keep = (x, ws)           # inputs stay alive until the caller synchronises on the result
         return out
-
-    def __del__(self):
-        try:
-            if getattr(self, "_handle", None):
-                self._lib.lspr_destroy(self._handle)
-                self._handle = C.c_void_p()
-        except Exception:
-            pass
 
 
 class ApcEncoder(_Recurrent):
     """``APC_encoder`` on one clip.  ``state_dict`` uses its key grammar (``rnns.{i}.weight_ih_l0``, ...; an optional
     ``module.`` prefix is accepted); the layer count and mel width are read from it.  ``device=-1`` makes a host-only
     handle (packing introspection)."""
+    what = "the APC encoder"
 
     def __init__(self, state_dict: Dict[str, torch.Tensor], device=None, residual: bool = False):
         sd = {k[7:] if k.startswith("module.") else k: v for k, v in state_dict.items()}
@@ -136,6 +105,7 @@ def mouth_output_size(opt) -> int:
 class MouthGenerator(_Recurrent):
     """Audio2Mouth: ``Audio2Feature`` with ``feature_decoder='LSTM'`` as ``generate_sequences`` runs it.  ``state_dict``
     uses its key grammar (``downsample.0.weight``, ``LSTM.weight_ih_l0``, ``fc.1.running_var``, ...)."""
+    what = "Audio2Mouth"
 
     def __init__(self, opt, state_dict: Dict[str, torch.Tensor], device=None):
         if getattr(opt, "feature_decoder", "LSTM") != "LSTM":
@@ -167,23 +137,6 @@ _APC: "Dict[int, tuple]" = {}          # id(module) -> (ApcEncoder, stamp)
 _MOUTH: "Dict[int, tuple]" = {}        # id(module) -> (MouthGenerator, stamp)
 
 
-def _cached(cache: dict, net, make, extra=()):
-    """The handle for ``net``, re-packed when its tensors changed: version counters move on every in-place write
-    (load_state_dict, optimiser steps), data pointers on re-allocation (``.to()``)."""
-    sd = net.state_dict()
-    stamp = (tuple((v.data_ptr(), v._version) for v in sd.values()), tuple(extra))
-    hit = cache.get(id(net))
-    if hit is None or hit[1] != stamp:
-        if hit is not None and hit[1][1] == stamp[1]:
-            gen = hit[0]
-            gen.load_state_dict(sd)
-        else:
-            gen = make(sd)
-        cache.clear()
-        cache[id(net)] = (gen, stamp)
-    return cache[id(net)][0]
-
-
 def apc_forward(self, inputs, lengths):
     """Replacement for ``APC_encoder.forward`` (models/networks.py:37-69), bound by ``install()``: inputs
     [1, T, mel_dim] on a CUDA device, lengths [T] -> [1, T, hidden] fp32 on the input's device."""
@@ -194,7 +147,7 @@ def apc_forward(self, inputs, lengths):
     lens = torch.as_tensor(lengths).reshape(-1)
     if lens.numel() != 1 or int(lens[0]) != inputs.shape[1]:
         raise ValueError(f"H100 APC encoder: lengths must be [{inputs.shape[1]}] (the full clip), got {lens.tolist()}")
-    enc = _cached(_APC, self, lambda sd: ApcEncoder(sd, inputs.device, residual=bool(self.rnn_residual)),
+    enc = _lib.cached(_APC, self, lambda sd: ApcEncoder(sd, inputs.device, residual=bool(self.rnn_residual)),
                   (bool(self.rnn_residual), str(inputs.device)))
     return enc.forward(inputs[0])[None]
 
@@ -215,7 +168,7 @@ def generate_sequences(self, audio_feats, sample_rate=16000, fps=60, fill_zero=T
     def make(sd):
         o = _OptView(mopt, frame_future=ff)
         return MouthGenerator(o, sd, device)
-    gen = _cached(_MOUTH, net, make, (ff, str(device)))
+    gen = _lib.cached(_MOUTH, net, make, (ff, str(device)))
     feats = torch.as_tensor(np.asarray(audio_feats)).to(device=device, dtype=torch.float32)
     return gen.generate(feats).cpu().numpy()                                            # :147-149
 

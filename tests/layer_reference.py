@@ -343,11 +343,8 @@ class Net:
             _lib.check(self.lib.lspg_layer_info_get(self.h, i, C.byref(info)))
             self.layers.append(info)
         if sd is not None:
-            keep = [(k.encode(), v.float().contiguous()) for k, v in sd.items() if not k.endswith("num_batches_tracked")]
-            arr = (_lib.LspgTensor * len(keep))()
-            for i, (k, t) in enumerate(keep):
-                arr[i].name, arr[i].numel, arr[i].data = k, t.numel(), C.cast(t.data_ptr(), C.POINTER(C.c_float))
-            _lib.check(self.lib.lspg_load_weights(self.h, arr, len(keep)))
+            arr, _keep = _lib.tensor_array(sd)
+            _lib.check(self.lib.lspg_load_weights(self.h, arr, len(arr)))
 
     def geo(self, i, b, hh, ww):
         g = _lib.LspgLayerGeo()
