@@ -40,6 +40,15 @@ int lspa_load_mel_basis(lspa_handle h, const float* host_basis, int n_mels, int 
 int lspa_logmel(lspa_handle h, const float* audio, int64_t n_samples, int n_windows, int frame_len, double step,
                 int normalize, float* out, void* stream);
 
+/* lspa_logmel on a piece of a clip, for streaming: audio holds the clip's samples [first_sample, first_sample + n_samples)
+ * and out receives windows first_window .. first_window + n_windows - 1 (window i still starts at (int64_t)(i * step),
+ * i the index in the whole clip).  Samples at or past first_sample + n_samples read as zero, which is the clip's end
+ * padding, so a caller passes a window that reaches past the samples it has only once the clip has ended.  The results
+ * are bit-identical to the same rows of lspa_logmel on the whole clip.  LSPG_EINVAL when window first_window starts
+ * before first_sample, or for first_sample < 0, first_window < 0 or first_window + n_windows >= 2^31. */
+int lspa_logmel_at(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
+                   int n_windows, int frame_len, double step, int normalize, float* out, void* stream);
+
 int lspa_destroy(lspa_handle h);
 const char* lspa_last_error(void);
 

@@ -67,6 +67,34 @@ int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n);
 int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
                   const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream);
 
+/* Bytes of the state of one stream (works on a host-only handle): fp32 [L][ring][residual_ch] history ring - the input of
+ * block l at absolute step t sits in slot t mod ring, ring the smallest power of two above the largest dilation (128 for
+ * the shipped options) - then 32 floats holding the network input of the next step (the last sample). */
+int lsph_state_bytes(lsph_handle h, size_t* bytes);
+
+/* Bytes of device workspace lsph_generate_stream needs for n_audio audio rows. */
+int lsph_stream_workspace_bytes(lsph_handle h, int n_audio, size_t* bytes);
+
+/* One chunk of a stream: frames frame0 .. frame0 + n_frames - 1 of the head-pose track.  Calls with consecutive frame
+ * ranges starting at 0 give, concatenated, the rows lsph_generate returns for the whole clip, bit for bit: the hoisted
+ * GEMMs are computed row by row and the loop runs the same steps in the same order.
+ *   audio_feats  [n_audio, 2*apc_hidden]: the clip's audio rows audio_row0 .. audio_row0 + n_audio - 1.  They must cover
+ *                rows frame0 + frame_future .. frame0 + n_frames - 1 + frame_future, and from row 0 when frame0 == 0
+ *                (the rf - 1 warm-up steps that replay window 0 read rows 0 .. frame_future - 1).  Frame i needs audio
+ *                up to row i + frame_future and nothing later.
+ *   noise        [n_frames, ndim], uniform [n_frames] or NULL: the draws of frames frame0 .. (as for lsph_generate)
+ *   out_pred     [n_frames, ndim], out_params [n_frames, out_ch] or NULL
+ *   state        lsph_state_bytes of caller-owned device memory, 16-byte aligned.  frame0 == 0 starts the loop from
+ *                pre_headpose (the ring needs no clearing: reads before step 0 are window 0's zero padding); every call
+ *                leaves the state after its last frame, which the call for frame0 + n_frames continues from.
+ *   ws           lsph_stream_workspace_bytes(h, n_audio) bytes, 256-byte aligned.
+ * n_frames == 0 does nothing.  LSPG_EINVAL (checked before the device, so also on a host-only handle) for a null state or
+ * audio rows that do not cover the frames; LSPG_ENODEV on a host-only handle.  Asynchronous on `stream`. */
+int lsph_generate_stream(lsph_handle h, const float* audio_feats, int audio_row0, int n_audio, int frame0, int n_frames,
+                         const float* pre_headpose, const float* noise, const float* uniform, float sigma_scale,
+                         float* out_pred, float* out_params, float* state, void* ws, size_t ws_bytes, int cluster,
+                         void* stream);
+
 /* Receptive field of the configured WaveNet (networks.py:147,175-176); 255 for the shipped options. */
 int lsph_receptive_field(lsph_handle h, int* out);
 

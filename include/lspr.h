@@ -66,6 +66,25 @@ int lspr_workspace_bytes(lspr_handle h, int n_rows, size_t* bytes);
  * 8 or 16, MOUTH 8.  Asynchronous on `stream`. */
 int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* ws, size_t ws_bytes, int cluster, void* stream);
 
+/* Bytes of the recurrent state of one stream: fp32 [num_layers][2][hidden], each layer's h and (LSTM) c.  Works on a
+ * host-only handle. */
+int lspr_state_bytes(lspr_handle h, size_t* bytes);
+
+/* One chunk of a stream: the clip's input rows pushed in pieces.  The chunks' outputs, concatenated, are bit-identical to
+ * lspr_forward on the whole clip, because the input projections and MLPs are computed row by row and every recurrent step
+ * is the same arithmetic whether it starts a launch or not.  state: lspr_state_bytes of caller-owned device memory, 16-byte
+ * aligned, carried from call to call; step0 == 0 zeroes it (h_0 = c_0 = 0) and every call replaces it with the state after
+ * its last step.
+ *   APC    in: rows step0 .. step0 + n_rows - 1 of the mel frames -> out [n_rows, hidden].
+ *   MOUTH  in: n_rows (even, >= 0) APC rows, the pairs step0 .. step0 + n_rows/2 - 1 -> out: the track rows of the global
+ *          LSTM steps max(step0, frame_future) .. step0 + n_rows/2 - 1, row s - frame_future for step s.  To end a clip of
+ *          n APC rows, pass 2 * frame_future copies of its last row with step0 = n / 2: that yields its last frame_future
+ *          track rows (models/audio2feature_model.py:134).
+ * ws: lspr_workspace_bytes(h, n_rows) bytes, cluster as for lspr_forward.  LSPG_EINVAL for a null state or an odd MOUTH
+ * row count (checked before the device, so also on a host-only handle); LSPG_ENODEV on a host-only handle. */
+int lspr_forward_stream(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
+                        size_t ws_bytes, int cluster, void* stream);
+
 /* Introspection (tests; works on a host-only handle): the arrays lspr_load_weights packed, as the kernels read them.
  * G = 3 (GRU: r, z, n) or 4 (LSTM: i, f, g, o), H = hidden units of the layer, In = its input width.  Gate rows are
  * interleaved by unit: packed row u*G + g is torch's row g*H + u, so the rows of units [c*H/CL, (c+1)*H/CL) - those

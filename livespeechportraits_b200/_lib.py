@@ -97,6 +97,9 @@ ARGTYPES = {
     "lsph_create": [_out_handle, C.POINTER(LsphConfig), _i],
     "lsph_load_weights": [_p, _tensors, _i],
     "lsph_generate": [_p, _p, _i, _p, _p, _p, C.c_float, _p, _p, _i, _p],
+    "lsph_state_bytes": [_p, _psz],
+    "lsph_stream_workspace_bytes": [_p, _i, _psz],
+    "lsph_generate_stream": [_p, _p, _i, _i, _i, _i, _p, _p, _p, C.c_float, _p, _p, _p, _p, _sz, _i, _p],
     "lsph_receptive_field": [_p, _pi],
     "lsph_debug_packed": [_p, _i, _p, _i64],
     "lsph_destroy": [_p],
@@ -113,6 +116,7 @@ ARGTYPES = {
     "lspa_create": [_out_handle, _i],
     "lspa_load_mel_basis": [_p, _p, _i, _i],
     "lspa_logmel": [_p, _p, _i64, _i, _i, C.c_double, _i, _p, _p],
+    "lspa_logmel_at": [_p, _p, _i64, _i64, _i, _i, _i, C.c_double, _i, _p, _p],
     "lspa_destroy": [_p],
     "lspa_last_error": [],
     # include/lspl.h (landmark post-processing, demo.py stage 5)
@@ -127,6 +131,8 @@ ARGTYPES = {
     "lspr_load_weights": [_p, _tensors, _i],
     "lspr_workspace_bytes": [_p, _i, _psz],
     "lspr_forward": [_p, _p, _i, _p, _p, _sz, _i, _p],
+    "lspr_state_bytes": [_p, _psz],
+    "lspr_forward_stream": [_p, _p, _i, _i64, _p, _p, _p, _sz, _i, _p],
     "lspr_debug_packed": [_p, _i, _p, _pi64],
     "lspr_destroy": [_p],
     "lspr_last_error": [],
@@ -204,6 +210,25 @@ def cuda_device(device, what: str) -> torch.device:
     return device if device.index is not None else torch.device("cuda", torch.cuda.current_device())
 
 
+def to_device(x, device: torch.device, dtype=torch.float32) -> torch.Tensor:
+    """``x`` (numpy, torch, any device) as a contiguous ``dtype`` tensor on ``device``.  A host array goes through pinned
+    memory with a non-blocking copy, so the call does not wait for the device (a pageable copy would)."""
+    t = torch.as_tensor(x)
+    if t.device.type == "cpu":
+        t = t.to(dtype=dtype).contiguous().pin_memory()
+        return t.to(device=device, non_blocking=True)
+    return t.to(device=device, dtype=dtype).contiguous()
+
+
+def reserve(buf: Optional[torch.Tensor], nbytes: int, device: torch.device) -> torch.Tensor:
+    """``buf`` if it holds at least ``nbytes`` bytes, else a new uint8 device buffer of ``nbytes`` (at least one byte).
+    A stream keeps its workspaces this way: after its largest push nothing is allocated per push, so its device memory
+    stays the same from push to push."""
+    if buf is None or buf.numel() < nbytes:
+        buf = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=device)
+    return buf
+
+
 def tensor_array(state_dict) -> Tuple[C.Array, list]:
     """A state dict as the ``lspg_tensor`` array of the ``*_load_weights`` calls: fp32 contiguous CPU copies, without
     BatchNorm's ``num_batches_tracked``.  The array points into ``keep``, which must outlive the call."""
@@ -237,7 +262,8 @@ def cached(cache: dict, net, make, extra=()):
 class Handle:
     """Owns one native handle of the C ABI ``<prefix>_*``: ``__init__`` resolves the device (-1: a host-only handle,
     ``self.device`` None), ``_create`` calls ``<prefix>_create(&handle, *args, device)``, ``call`` makes checked calls
-    with the handle first, and ``__del__`` destroys it."""
+    with the handle first, ``cuda_stream`` enters the device and yields its current CUDA stream, and ``__del__``
+    destroys it.  (``stream()`` on the subclasses opens an audio stream.)"""
     prefix = ""
     what = ""                      # names the subclass in the "no CPU path" refusal
     _handle = None
@@ -256,16 +282,20 @@ class Handle:
         check(getattr(self._lib, f"{self.prefix}_{name}")(self._handle, *args), self.prefix)
 
     @contextlib.contextmanager
-    def stream(self):
+    def cuda_stream(self):
         """Enters the handle's device and yields its current stream (a ``cudaStream_t`` as int)."""
         with torch.cuda.device(self.device):
             yield torch.cuda.current_stream(self.device).cuda_stream
 
-    def workspace(self, *args) -> torch.Tensor:
-        """A device buffer of the ``<prefix>_workspace_bytes(handle, *args)`` bytes (at least one byte)."""
+    def workspace_bytes(self, *args) -> int:
+        """``<prefix>_workspace_bytes(handle, *args)``."""
         need = C.c_size_t()
         self.call("workspace_bytes", *args, C.byref(need))
-        return torch.empty(max(need.value, 1), dtype=torch.uint8, device=self.device)
+        return need.value
+
+    def workspace(self, *args) -> torch.Tensor:
+        """A device buffer of the ``<prefix>_workspace_bytes(handle, *args)`` bytes (at least one byte)."""
+        return torch.empty(max(self.workspace_bytes(*args), 1), dtype=torch.uint8, device=self.device)
 
     def __del__(self):
         try:

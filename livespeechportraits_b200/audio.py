@@ -121,9 +121,70 @@ class MelFrontEnd(_lib.Handle):
         a = a.to(device=self.device, dtype=torch.float32).contiguous()
         n = 2 * int(a.shape[0] / 16000 * 60)
         out = torch.empty((n, self.n_mels), dtype=torch.float32, device=self.device)
-        with self.stream() as stream:
+        with self.cuda_stream() as stream:
             self.call("logmel", a.data_ptr() if a.numel() else None, a.shape[0], n, frame_len, step, int(bool(normalize)),
                       out.data_ptr() if n else None, stream)
+        return out
+
+
+    def stream(self, winlen: float = 1 / 60, winstep: float = 0.5 / 60, sr: int = 16000,
+               normalize: bool = True) -> "MelStream":
+        """A stream over one clip's samples: ``push(samples)`` returns the windows that became complete, ``finish()`` the
+        rest.  The concatenation equals ``logmel`` of all the samples, bit for bit."""
+        return MelStream(self, winlen, winstep, sr, normalize)
+
+
+class MelStream:
+    """The log-mel frames of a clip pushed in pieces (``MelFrontEnd.stream``).  Window i is returned by the push that
+    completes its ``frame_len`` samples, once ``i < 2 int(n / 16000 * 60)`` for the n samples pushed so far
+    (``stream.mel_windows``); the windows that reach into the end padding come out at ``finish()``.  Only the samples
+    from the start of the next window on are kept on the device."""
+
+    def __init__(self, front: MelFrontEnd, winlen: float, winstep: float, sr: int, normalize: bool):
+        self._front = front
+        self.frame_len = frame_len_of(sr, winlen)
+        self.step = float(sr * winstep)
+        if not self.step > 0:
+            raise ValueError(f"the window step sr * winstep must be > 0 (got {self.step})")
+        self._normalize = int(bool(normalize))
+        self.samples = 0                       # samples pushed so far
+        self.windows = 0                       # windows returned so far
+        self.finished = False
+        self._tail = torch.empty(0, dtype=torch.float32, device=front.device)   # samples tail0 .. samples - 1
+        self._tail0 = 0
+
+    def push(self, samples) -> torch.Tensor:
+        """1-D samples (numpy or torch, any float dtype, any device; 16 kHz mono) -> the new windows [m, n_mels] CUDA."""
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        a = _lib.to_device(samples, self._front.device)
+        if a.dim() != 1:
+            raise ValueError(f"samples must be 1-D, got shape {tuple(a.shape)}")
+        self.samples += a.shape[0]
+        buf = torch.cat([self._tail, a]) if self._tail.numel() else a
+        return self._emit(buf, False)
+
+    def finish(self) -> torch.Tensor:
+        """The windows that need the end padding."""
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        self.finished = True
+        return self._emit(self._tail, True)
+
+    def _emit(self, buf: torch.Tensor, finished: bool) -> torch.Tensor:
+        from .stream import mel_windows
+        ready = mel_windows(self.samples, finished, self.frame_len, self.step)
+        k = ready - self.windows
+        out = torch.empty((k, self._front.n_mels), dtype=torch.float32, device=self._front.device)
+        if k:
+            with self._front.cuda_stream() as stream:
+                self._front.call("logmel_at", buf.data_ptr() if buf.numel() else None, self._tail0, buf.shape[0], self.windows,
+                                 k, self.frame_len, self.step, self._normalize, out.data_ptr(), stream)
+        self.windows = ready
+        keep = min(int(self.windows * self.step), self.samples)        # where the next window starts
+        self._tail = buf[keep - self._tail0:].clone()
+        self._tail0 = keep
+        self._keep = buf
         return out
 
 

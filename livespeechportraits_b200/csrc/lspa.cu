@@ -54,8 +54,11 @@ struct Smem {
 static_assert(kWin * kMaxMels <= kWinLen * kWin, "output stage must fit in the frame buffer");
 static_assert(2 * kMaxMels <= kThreads, "one thread per (mel, half of the windows)");
 
-__global__ void __launch_bounds__(kThreads) lspa_logmel_kernel(const float* __restrict__ audio, int64_t n_samples,
-                                                               int n_windows, int frame_len, double step,
+// audio holds clip samples [first_sample, first_sample + n_samples); samples past its end read as zero (the clip's end
+// padding).  Block b computes windows first_window + b*kWin ..., stored from out row b*kWin.
+__global__ void __launch_bounds__(kThreads) lspa_logmel_kernel(const float* __restrict__ audio, int64_t first_sample,
+                                                               int64_t n_samples, int first_window, int n_windows,
+                                                               int frame_len, double step,
                                                                const float2* __restrict__ tw_g, const float* __restrict__ hann_g,
                                                                const float* __restrict__ basis, int n_mels, int normalize,
                                                                float* __restrict__ out) {
@@ -72,11 +75,11 @@ __global__ void __launch_bounds__(kThreads) lspa_logmel_kernel(const float* __re
     const int t = e / kWin, g = e % kWin;
     float v = 0.f;
     if (g < nw) {
-      const int64_t st = static_cast<int64_t>(__dmul_rn(static_cast<double>(w0 + g), step));
+      const int64_t st = static_cast<int64_t>(__dmul_rn(static_cast<double>(first_window + w0 + g), step));
       int p = t + kWinOff - kPad;
       if (p < 0) p = -p;
       if (p >= frame_len) p = 2 * (frame_len - 1) - p;
-      const int64_t a = st + p;
+      const int64_t a = st + p - first_sample;
       if (a < n_samples) v = __fmul_rn(sm.hann[t], __ldg(audio + a));
     }
     sm.frame[t][g] = v;
@@ -218,26 +221,44 @@ int lspa_load_mel_basis(lspa_handle h, const float* host_basis, int n_mels, int 
   return LSPG_OK;
 }
 
-int lspa_logmel(lspa_handle h, const float* audio, int64_t n_samples, int n_windows, int frame_len, double step,
-                int normalize, float* out, void* stream) {
+static int logmel(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
+                  int n_windows, int frame_len, double step, int normalize, float* out, void* stream, const char* what) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
   if (n_samples < 0) return fail(LSPG_EINVAL, "n_samples must be >= 0 (got %lld)", static_cast<long long>(n_samples));
   if (n_windows < 0) return fail(LSPG_EINVAL, "n_windows must be >= 0 (got %d)", n_windows);
   if (frame_len < kMinFrame || frame_len > kMaxFrame)
     return fail(LSPG_EINVAL, "frame_len must be in [%d, %d] (got %d): the reflect pad of %d needs a longer clip and one stft "
                  "frame a shorter one", kMinFrame, kMaxFrame, frame_len, kPad);
-  if (!(step >= 0.0) || !(step * static_cast<double>(n_windows) < 4.0e18))
+  if (!(step >= 0.0) || !(step * (static_cast<double>(first_window) + n_windows) < 4.0e18))
     return fail(LSPG_EINVAL, "step must be finite and >= 0, with n_windows * step < 4e18 (got %g)", step);
   if ((!audio && n_samples > 0) || (!out && n_windows > 0)) return fail(LSPG_EINVAL, "null buffer");
-  if (int rc = capi::require_device<Lspa>(h->device, "lspa_logmel")) return rc;
+  if (first_sample < 0 || first_window < 0 || static_cast<int64_t>(first_window) + n_windows > INT32_MAX)
+    return fail(LSPG_EINVAL, "first_sample and first_window must be >= 0, with first_window + n_windows < 2^31 (got %lld, %d)",
+                static_cast<long long>(first_sample), first_window);
+  if (n_windows > 0 && static_cast<int64_t>(static_cast<double>(first_window) * step) < first_sample)
+    return fail(LSPG_EINVAL, "window %d starts at sample %lld, before the first sample given (%lld)", first_window,
+                static_cast<long long>(static_cast<double>(first_window) * step), static_cast<long long>(first_sample));
+  if (int rc = capi::require_device<Lspa>(h->device, what)) return rc;
   if (h->n_mels == 0) return fail(LSPG_ESTATE, "lspa_load_mel_basis has not been called");
   if (n_windows == 0) return LSPG_OK;
   DeviceGuard g(h->device);
   const int blocks = n_windows / kWin + (n_windows % kWin != 0);   // w0 = blockIdx.x * kWin < n_windows < 2^31
   lspa_logmel_kernel<<<blocks, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      audio, n_samples, n_windows, frame_len, step, h->d_tw, h->d_hann, h->d_basis, h->n_mels, normalize ? 1 : 0, out);
+      audio, first_sample, n_samples, first_window, n_windows, frame_len, step, h->d_tw, h->d_hann, h->d_basis, h->n_mels,
+      normalize ? 1 : 0, out);
   CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
+}
+
+int lspa_logmel(lspa_handle h, const float* audio, int64_t n_samples, int n_windows, int frame_len, double step,
+                int normalize, float* out, void* stream) {
+  return logmel(h, audio, 0, n_samples, 0, n_windows, frame_len, step, normalize, out, stream, "lspa_logmel");
+}
+
+int lspa_logmel_at(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
+                   int n_windows, int frame_len, double step, int normalize, float* out, void* stream) {
+  return logmel(h, audio, first_sample, n_samples, first_window, n_windows, frame_len, step, normalize, out, stream,
+                "lspa_logmel_at");
 }
 
 }  // extern "C"

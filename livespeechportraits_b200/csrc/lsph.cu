@@ -61,15 +61,17 @@ struct LoopParams {
   const float* b_rs;       // [L][R + S]
   const float* w_end1; const float* b_end1;          // [O][S], [O]
   const float* w_end2; const float* b_end2;          // [O][O], [O]
-  const float* cond;       // [n_audio][L][2R]: cond_filter/gate conv of every audio row + their biases + filter/gate biases
+  const float* cond;       // [n_audio][L][2R]: cond_filter/gate conv of audio rows arow0 .. + their biases + filter/gate biases
+  const float* h_in;           // [in_ch]: the network input of step t0 (the last sample), or null: pre_headpose
   const float* pre_headpose;   // [in_ch]
-  const float* noise;          // [nframe][ndim]
-  const float* uniform;        // [nframe] or null
-  float* hist;                 // [L][T][R]: input of block l at absolute time t
-  float* out_pred;             // [nframe][ndim]
-  float* out_params;           // [nframe][O] or null
+  const float* noise;          // [n frames][ndim], row i - frame0 for frame i
+  const float* uniform;        // [n frames] or null
+  float* hist;                 // [L][ring][R]: input of block l at absolute time t, in slot t mod ring
+  float* h_out;                // [in_ch] or null: the network input after the last step
+  float* out_pred;             // [n frames][ndim]
+  float* out_params;           // [n frames][O] or null
   int L, in_ch, O, ndim, ncenter, gmm;
-  int n_audio, nframe, rf, ff, T;
+  int n_audio, arow0, frame0, rf, ff, t0, t1, ring;
   float sigma_scale;
   int dil[kMaxLayers];
 };
@@ -118,7 +120,7 @@ __global__ void __launch_bounds__(NW * 32, 1) headpose_loop_kernel(const LoopPar
   __shared__ __align__(16) float e1_s[kMaxOut];
   __shared__ __align__(16) float out_s[kMaxOut];
 
-  if (tid < p.in_ch) h_s[tid] = p.pre_headpose[tid];
+  if (tid < p.in_ch) h_s[tid] = p.h_in ? p.h_in[tid] : p.pre_headpose[tid];
   __syncthreads();
 
   float4 wa[kPrefetch ? kRowsA : 1][2];
@@ -154,15 +156,16 @@ __global__ void __launch_bounds__(NW * 32, 1) headpose_loop_kernel(const LoopPar
   load_a(0);
 
   int cur = 0;
-  for (int t = 0; t < p.T; ++t) {
+  for (int t = p.t0; t < p.t1; ++t) {
     const bool emit = t >= p.rf - 1;
-    int arow = t + p.ff - (p.rf - 1);
+    int arow = t + p.ff - (p.rf - 1);                  // absolute audio row, the first rf - 1 steps replay row 0 ...
+    arow = (arow < 0 ? 0 : arow) - p.arow0;            // ... relative to the first row given (the host checks coverage)
     arow = arow < 0 ? 0 : (arow > p.n_audio - 1 ? p.n_audio - 1 : arow);
     // ---- off the critical path: the delayed inputs of every block (written >= 1 step ago) and this step's conditioning terms
     for (int idx = tid; idx < p.L * kR; idx += NW * 32) {
       const int l = idx / kR, k = idx - l * kR;
       const int td = t - p.dil[l];
-      xd_all[l][k] = (td >= 0) ? p.hist[(static_cast<size_t>(l) * p.T + td) * kR + k] : 0.f;    // zero padding of window 0
+      xd_all[l][k] = (td >= 0) ? p.hist[(static_cast<size_t>(l) * p.ring + (td & (p.ring - 1))) * kR + k] : 0.f;  // zero padding of window 0
     }
     for (int idx = tid; idx < p.L * kOutA; idx += NW * 32) {
       const int l = idx / kOutA, o = idx - l * kOutA;
@@ -186,7 +189,7 @@ __global__ void __launch_bounds__(NW * 32, 1) headpose_loop_kernel(const LoopPar
     __syncthreads();
 
     for (int l = 0; l < p.L; ++l) {
-      if (crank == 0 && tid < kR) p.hist[(static_cast<size_t>(l) * p.T + t) * kR + tid] = xbuf[cur][tid];   // X[l][t]
+      if (crank == 0 && tid < kR) p.hist[(static_cast<size_t>(l) * p.ring + (t & (p.ring - 1))) * kR + tid] = xbuf[cur][tid];   // X[l][t]
       load_b(l);                                     // stage-B weight rows are in flight across stage A and barrier #1
       // ---- stage A: filter / gate pre-activations of this CTA's channels
       {
@@ -257,7 +260,7 @@ __global__ void __launch_bounds__(NW * 32, 1) headpose_loop_kernel(const LoopPar
     }
 
     if (emit) {
-      const int i = t - (p.rf - 1);
+      const int i = t - (p.rf - 1) - p.frame0;       // row of the frame in this launch's noise / outputs
       // ---- LeakyReLU(skip) of every CTA's channels -> rank 0
       if (tid < kSc) {
         const float v = lrelu(skip_acc[tid]);
@@ -319,6 +322,8 @@ __global__ void __launch_bounds__(NW * 32, 1) headpose_loop_kernel(const LoopPar
       if constexpr (CL > 1) cluster.sync(); else __syncthreads();                            // barrier #4: new history sample everywhere
     }
   }
+  // Every CTA read h_in before its first barrier, so it may be overwritten now.
+  if (p.h_out && crank == 0 && tid < p.in_ch) p.h_out[tid] = h_s[tid];
 }
 
 struct HostTensor {
@@ -332,6 +337,7 @@ struct lsph_ctx {
   lsph_config cfg{};
   int device = -1;
   int L = 0, O = 0, rf = 0;
+  int ring = 0;                      // history slots per layer: the smallest power of two above the largest dilation
   std::vector<int> dil;
   bool weights_loaded = false;
   // device weights
@@ -343,7 +349,7 @@ struct lsph_ctx {
   float *d_w_end1 = nullptr, *d_b_end1 = nullptr, *d_w_end2 = nullptr, *d_b_end2 = nullptr;
   // scratch (grown on demand)
   int cap_audio = 0;
-  float *d_ds1 = nullptr, *d_ds2 = nullptr, *d_cond = nullptr, *d_hist = nullptr;
+  float *d_ds1 = nullptr, *d_hist = nullptr;   // the hoisted path's workspace for cap_audio rows; the history ring
   std::vector<float*> owned;
   std::vector<float> packed[7];      // host copies of the packed arrays (lsph_debug_packed)
 };
@@ -387,6 +393,7 @@ int lsph_create(lsph_handle* out, const lsph_config* c, int device) {
   h->rf = 1;
   for (int b = 0; b < c->blocks; ++b)
     for (int i = 0; i < c->layers; ++i) { h->dil.push_back(1 << i); h->rf += (1 << i); }      // networks.py:160-176
+  h->ring = 2 << (c->layers - 1);
   cudaDeviceProp prop;
   if (int rc = capi::check_device<Lsph>(device, &prop)) return rc;
   *out = h.release();
@@ -404,7 +411,7 @@ int lsph_destroy(lsph_handle h) {
   if (h->device >= 0) {
     DeviceGuard g(h->device);
     for (float* p : h->owned) cudaFree(p);
-    for (float* p : {h->d_ds1, h->d_ds2, h->d_cond, h->d_hist})
+    for (float* p : {h->d_ds1, h->d_hist})
       if (p) cudaFree(p);
   }
   delete h;
@@ -516,48 +523,44 @@ int lsph_debug_packed(lsph_handle h, int which, float* dst, int64_t count) {
   return LSPG_OK;
 }
 
-int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
-                  const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream) {
-  if (!h) return fail(LSPG_EINVAL, "null handle");
-  if (int rc = capi::require_device<Lsph>(h->device, "lsph_generate")) return rc;
-  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lsph_load_weights has not been called");
+// Workspace of the hoisted audio path for n_audio rows (floats, every block 64-float aligned): ds1, ds2 [n][H], cond [n][L][2R].
+static size_t hoisted_floats(const lsph_ctx* h, int n_audio, size_t off[3]) {
+  const size_t n = static_cast<size_t>(n_audio), sz[3] = {n * h->cfg.apc_hidden, n * h->cfg.apc_hidden, n * h->L * 2 * kR};
+  size_t total = 0;
+  for (int i = 0; i < 3; ++i) { off[i] = total; total += (sz[i] + 63) / 64 * 64; }
+  return total;
+}
+
+static size_t state_floats(const lsph_ctx* h) { return static_cast<size_t>(h->L) * h->ring * kR + kMaxIn; }
+
+// Frames frame0 .. frame0 + n_frames - 1 (absolute steps from t0 = frame0 + rf - 1, or from 0 with the warm-up when
+// frame0 == 0) from audio rows arow0 .. arow0 + n_audio - 1.  h_state null: pre_headpose starts the loop and nothing is saved.
+static int run(lsph_handle h, const float* audio_feats, int arow0, int n_audio, int frame0, int n_frames,
+               const float* pre_headpose, const float* noise, const float* uniform, float sigma_scale, float* out_pred,
+               float* out_params, float* hist, float* h_state, float* ws, int cluster, cudaStream_t st) {
   const lsph_config& c = h->cfg;
-  if (!audio_feats || !pre_headpose || !out_pred) return fail(LSPG_EINVAL, "null buffer");
-  if (c.loss_gmm && !noise) return fail(LSPG_EINVAL, "noise is required for the GMM loss (pass zeros for sigma_scale 0)");
-  const int nframe = n_audio - c.frame_future;
-  if (nframe < 1) return fail(LSPG_EINVAL, "need more than frame_future (%d) audio rows, got %d", c.frame_future, n_audio);
-  if (cluster == 0) cluster = 8;
-  if (cluster != 1 && cluster != 8) return fail(LSPG_EINVAL, "cluster must be 1 or 8 (got %d)", cluster);
-  DeviceGuard g(h->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int H = c.apc_hidden, L = h->L, T = h->rf - 1 + nframe;
-  if (n_audio > h->cap_audio) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    for (float** p : {&h->d_ds1, &h->d_ds2, &h->d_cond, &h->d_hist})
-      if (*p) { cudaFree(*p); *p = nullptr; }
-    const int cap = n_audio + 64;
-    CUDA_TRY(cudaMalloc(&h->d_ds1, sizeof(float) * static_cast<size_t>(cap) * H));
-    CUDA_TRY(cudaMalloc(&h->d_ds2, sizeof(float) * static_cast<size_t>(cap) * H));
-    CUDA_TRY(cudaMalloc(&h->d_cond, sizeof(float) * static_cast<size_t>(cap) * L * 2 * kR));
-    CUDA_TRY(cudaMalloc(&h->d_hist, sizeof(float) * static_cast<size_t>(L) * (h->rf - 1 + cap) * kR));
-    h->cap_audio = cap;
-  }
-  // ---- hoisted audio path: downsample every row, project it for every block
+  const int H = c.apc_hidden, L = h->L;
+  size_t off[3];
+  hoisted_floats(h, n_audio, off);
+  float *ds1 = ws + off[0], *ds2 = ws + off[1], *cond = ws + off[2];
+  // ---- hoisted audio path: downsample every row given, project it for every block
   const dim3 blk(256);
   const int mt = (n_audio + 63) / 64;
-  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, h->d_ds1, n_audio, H, 2 * H, 1, 0);
-  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(h->d_ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, h->d_ds2, n_audio, H, H, 0, 0);
-  gemm_nt_kernel<><<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(h->d_ds2, h->d_w_cond, h->d_one, h->d_b_cond, h->d_cond, n_audio, L * 2 * kR, H, 0, 0);
+  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, ds1, n_audio, H, 2 * H, 1, 0);
+  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, ds2, n_audio, H, H, 0, 0);
+  gemm_nt_kernel<><<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(ds2, h->d_w_cond, h->d_one, h->d_b_cond, cond, n_audio, L * 2 * kR, H, 0, 0);
   CUDA_TRY(cudaGetLastError());
   LoopParams p;
   memset(&p, 0, sizeof(p));
   p.w_start1 = h->d_w_start1; p.b_start1 = h->d_b_start1; p.w_start2 = h->d_w_start2; p.b_start2 = h->d_b_start2;
   p.w_fg = h->d_w_fg; p.w_rs = h->d_w_rs; p.b_rs = h->d_b_rs;
   p.w_end1 = h->d_w_end1; p.b_end1 = h->d_b_end1; p.w_end2 = h->d_w_end2; p.b_end2 = h->d_b_end2;
-  p.cond = h->d_cond; p.pre_headpose = pre_headpose; p.noise = noise; p.uniform = uniform;
-  p.hist = h->d_hist; p.out_pred = out_pred; p.out_params = out_params;
+  p.cond = cond; p.h_in = (h_state && frame0 > 0) ? h_state : nullptr; p.pre_headpose = pre_headpose;
+  p.noise = noise; p.uniform = uniform;
+  p.hist = hist; p.h_out = h_state; p.out_pred = out_pred; p.out_params = out_params;
   p.L = L; p.in_ch = c.input_ch; p.O = h->O; p.ndim = c.ndim; p.ncenter = c.ncenter; p.gmm = c.loss_gmm;
-  p.n_audio = n_audio; p.nframe = nframe; p.rf = h->rf; p.ff = c.frame_future; p.T = T;
+  p.n_audio = n_audio; p.arow0 = arow0; p.frame0 = frame0; p.rf = h->rf; p.ff = c.frame_future;
+  p.t0 = frame0 == 0 ? 0 : frame0 + h->rf - 1; p.t1 = frame0 + n_frames + h->rf - 1; p.ring = h->ring;
   p.sigma_scale = sigma_scale;
   for (int l = 0; l < L; ++l) p.dil[l] = h->dil[l];
   if (cluster == 8) {
@@ -573,6 +576,83 @@ int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const fl
     CUDA_TRY(cudaGetLastError());
   }
   return LSPG_OK;
+}
+
+int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
+                  const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream) {
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (int rc = capi::require_device<Lsph>(h->device, "lsph_generate")) return rc;
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lsph_load_weights has not been called");
+  const lsph_config& c = h->cfg;
+  if (!audio_feats || !pre_headpose || !out_pred) return fail(LSPG_EINVAL, "null buffer");
+  if (c.loss_gmm && !noise) return fail(LSPG_EINVAL, "noise is required for the GMM loss (pass zeros for sigma_scale 0)");
+  const int nframe = n_audio - c.frame_future;
+  if (nframe < 1) return fail(LSPG_EINVAL, "need more than frame_future (%d) audio rows, got %d", c.frame_future, n_audio);
+  if (cluster == 0) cluster = 8;
+  if (cluster != 1 && cluster != 8) return fail(LSPG_EINVAL, "cluster must be 1 or 8 (got %d)", cluster);
+  DeviceGuard g(h->device);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n_audio > h->cap_audio) {
+    CUDA_TRY(cudaDeviceSynchronize());
+    if (h->d_ds1) { cudaFree(h->d_ds1); h->d_ds1 = nullptr; }
+    const int cap = n_audio + 64;
+    size_t off[3];
+    CUDA_TRY(cudaMalloc(&h->d_ds1, sizeof(float) * hoisted_floats(h, cap, off)));
+    if (!h->d_hist) CUDA_TRY(cudaMalloc(&h->d_hist, sizeof(float) * state_floats(h)));
+    h->cap_audio = cap;
+  }
+  return run(h, audio_feats, 0, n_audio, 0, nframe, pre_headpose, noise, uniform, sigma_scale, out_pred, out_params, h->d_hist,
+             nullptr, h->d_ds1, cluster, st);
+}
+
+int lsph_state_bytes(lsph_handle h, size_t* bytes) {
+  if (!h || !bytes) return fail(LSPG_EINVAL, "null argument");
+  *bytes = sizeof(float) * state_floats(h);
+  return LSPG_OK;
+}
+
+int lsph_stream_workspace_bytes(lsph_handle h, int n_audio, size_t* bytes) {
+  if (!h || !bytes) return fail(LSPG_EINVAL, "null argument");
+  if (n_audio < 0) return fail(LSPG_EINVAL, "n_audio must be >= 0 (got %d)", n_audio);
+  size_t off[3];
+  *bytes = sizeof(float) * hoisted_floats(h, n_audio, off);
+  return LSPG_OK;
+}
+
+int lsph_generate_stream(lsph_handle h, const float* audio_feats, int audio_row0, int n_audio, int frame0, int n_frames,
+                         const float* pre_headpose, const float* noise, const float* uniform, float sigma_scale,
+                         float* out_pred, float* out_params, float* state, void* ws, size_t ws_bytes, int cluster,
+                         void* stream) {
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  const lsph_config& c = h->cfg;
+  if (!state) return fail(LSPG_EINVAL, "null state");
+  if (frame0 < 0 || n_frames < 0 || audio_row0 < 0 || n_audio < 0)
+    return fail(LSPG_EINVAL, "frame0, n_frames, audio_row0 and n_audio must be >= 0 (got %d, %d, %d, %d)", frame0, n_frames,
+                audio_row0, n_audio);
+  const int64_t lo = frame0 == 0 ? 0 : static_cast<int64_t>(frame0) + c.frame_future;   // frame 0 also replays rows 0 ..
+  const int64_t hi = static_cast<int64_t>(frame0) + n_frames + c.frame_future;           // exclusive
+  if (hi + h->rf > INT32_MAX) return fail(LSPG_EINVAL, "frame0 + n_frames is too large");
+  if (n_frames > 0 && (audio_row0 > lo || static_cast<int64_t>(audio_row0) + n_audio < hi))
+    return fail(LSPG_EINVAL, "frames %d .. %d need audio rows %lld .. %lld, the rows given are %d .. %lld", frame0,
+                frame0 + n_frames - 1, static_cast<long long>(lo), static_cast<long long>(hi - 1), audio_row0,
+                static_cast<long long>(audio_row0) + n_audio - 1);
+  if (n_frames > 0 && (!audio_feats || !pre_headpose || !out_pred)) return fail(LSPG_EINVAL, "null buffer");
+  if (n_frames > 0 && c.loss_gmm && !noise) return fail(LSPG_EINVAL, "noise is required for the GMM loss (pass zeros for sigma_scale 0)");
+  if (reinterpret_cast<uintptr_t>(state) % 16) return fail(LSPG_EINVAL, "state must be 16-byte aligned");
+  size_t off[3];
+  const size_t need = n_frames > 0 ? sizeof(float) * hoisted_floats(h, n_audio, off) : 0;
+  if (ws_bytes < need) return fail(LSPG_EINVAL, "workspace of %zu bytes is smaller than the %zu needed", ws_bytes, need);
+  if (need && (!ws || reinterpret_cast<uintptr_t>(ws) % 256)) return fail(LSPG_EINVAL, "workspace must be non-null and 256-byte aligned");
+  if (cluster == 0) cluster = 8;
+  if (cluster != 1 && cluster != 8) return fail(LSPG_EINVAL, "cluster must be 1 or 8 (got %d)", cluster);
+  if (int rc = capi::require_device<Lsph>(h->device, "lsph_generate_stream")) return rc;
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lsph_load_weights has not been called");
+  if (n_frames == 0) return LSPG_OK;
+  DeviceGuard g(h->device);
+  float* hist = state;
+  float* h_state = state + static_cast<size_t>(h->L) * h->ring * kR;
+  return run(h, audio_feats, audio_row0, n_audio, frame0, n_frames, pre_headpose, noise, uniform, sigma_scale, out_pred,
+             out_params, hist, h_state, static_cast<float*>(ws), cluster, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

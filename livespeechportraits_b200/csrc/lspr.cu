@@ -51,6 +51,7 @@ struct RecParams {
   const float* b_hn;    // [H] (GRU) or null
   const float* resid;   // [T][H] added to the output (APC residual), or null
   float* out;           // [T][H]
+  float* state;         // [2][H]: h (and the LSTM's c) before step 0, replaced by their values after step T-1; or null (zeros)
   int T;
 };
 
@@ -90,9 +91,10 @@ __global__ void __launch_bounds__(kNW * 32, 1) rnn_layer_kernel(const RecParams 
 
   for (int i = tid; i < RS * H / 4; i += kNW * 32)
     reinterpret_cast<float4*>(w_s)[i] = __ldg(reinterpret_cast<const float4*>(w_cta) + i);
-  for (int i = tid; i < 2 * H; i += kNW * 32) h_s[i] = 0.f;             // h_0 = 0 (and c_0 = 0 below)
+  for (int i = tid; i < 2 * H; i += kNW * 32) h_s[i] = (p.state && i < H) ? p.state[i] : 0.f;   // h_0 = 0 or the saved h
   const int u = c * U + tid;                                            // the unit this thread updates (tid < U)
-  float cst = 0.f;
+  float cst = (G == 4 && p.state && tid < U) ? p.state[H + u] : 0.f;    // c_0 likewise
+  float hlast = 0.f;
   float bhn = 0.f;
   float xg[G];
   if (tid < U) {
@@ -147,6 +149,7 @@ __global__ void __launch_bounds__(kNW * 32, 1) rnn_layer_kernel(const RecParams 
       for (int r = 0; r < CL; ++r) cluster.map_shared_rank(h_s, r)[(cur ^ 1) * H + u] = hn;
       const size_t o = static_cast<size_t>(t) * H + u;
       p.out[o] = p.resid ? hn + p.resid[o] : hn;
+      hlast = hn;
       if (t + 1 < p.T) {
 #pragma unroll
         for (int g = 0; g < G; ++g) xg[g] = __ldg(p.xproj + (static_cast<size_t>(t + 1) * H + u) * G + g);
@@ -154,6 +157,11 @@ __global__ void __launch_bounds__(kNW * 32, 1) rnn_layer_kernel(const RecParams 
     }
     cluster.sync();                  // h_t complete in every CTA
     cur ^= 1;
+  }
+  // Every CTA read the saved state before the first step's barrier, so the units' owners may now replace it.
+  if (p.state && p.T > 0 && tid < U) {
+    p.state[u] = hlast;
+    if constexpr (G == 4) p.state[H + u] = cst;
   }
 }
 
@@ -411,17 +419,36 @@ int lspr_workspace_bytes(lspr_handle h, int n_rows, size_t* bytes) {
   return LSPG_OK;
 }
 
-int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* ws, size_t ws_bytes, int cluster, void* stream) {
+int lspr_state_bytes(lspr_handle h, size_t* bytes) {
+  if (!h || !bytes) return fail(LSPG_EINVAL, "null argument");
+  *bytes = sizeof(float) * static_cast<size_t>(h->L) * 2 * h->H;      // [L][2][H]: h, then c (LSTM; unused by the GRU)
+  return LSPG_OK;
+}
+
+// The whole clip (state == nullptr: every layer starts from zeros, Audio2Mouth appends its frame_future pairs of the last
+// row) or one chunk of a stream (state: the layers' h and c, carried across calls; step0: global step of the chunk's first
+// row, APC, or pair, MOUTH).
+static int forward(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
+                   size_t ws_bytes, int cluster, void* stream, const char* what) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
-  if (int rc = capi::require_device<Lspr>(h->device, "lspr_forward")) return rc;
-  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
   const lspr_config& c = h->cfg;
   const bool apc = c.kind == LSPR_APC;
-  if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
-  if (!apc && (n_rows < 2 || n_rows % 2))
-    return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even and >= 2 (got %d)", n_rows);
-  if (n_rows > 0 && (!in || !out)) return fail(LSPG_EINVAL, "null buffer");
-  if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out)) % 16) return fail(LSPG_EINVAL, "in and out must be 16-byte aligned");
+  if (!state) {
+    if (int rc = capi::require_device<Lspr>(h->device, what)) return rc;
+    if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
+    if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
+    if (!apc && (n_rows < 2 || n_rows % 2))
+      return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even and >= 2 (got %d)", n_rows);
+  } else {
+    if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
+    if (!apc && n_rows % 2) return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even (got %d)", n_rows);
+    if (step0 < 0 || step0 > INT32_MAX) return fail(LSPG_EINVAL, "step0 must be in [0, 2^31) (got %lld)", static_cast<long long>(step0));
+  }
+  // a MOUTH chunk before frame_future returns no rows, so it may pass no output buffer
+  if (n_rows > 0 && (!in || (!out && (apc || !state || step0 + n_rows / 2 > c.frame_future))))
+    return fail(LSPG_EINVAL, "null buffer");
+  if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(state)) % 16)
+    return fail(LSPG_EINVAL, "in, out and state must be 16-byte aligned");
   size_t off[5];
   const size_t need = sizeof(float) * workspace_floats(h, n_rows, off);
   if (ws_bytes < need) return fail(LSPG_EINVAL, "workspace of %zu bytes is smaller than the %zu needed", ws_bytes, need);
@@ -434,18 +461,24 @@ int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* w
     if (cl == 0) cl = 8;
     if (cl != 8) return fail(LSPG_EINVAL, "Audio2Mouth cluster must be 0 or 8 (got %d)", cluster);
   }
+  if (state) {
+    if (int rc = capi::require_device<Lspr>(h->device, what)) return rc;
+    if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
+  }
   if ((cl == 16 ? h->max_clusters16 : h->max_clusters8) < 1)
     return fail(LSPG_ENODEV, "a %d-CTA cluster with %zu bytes of shared memory per CTA cannot be scheduled on device %d", cl,
                  cl == 16 ? kGru16Smem : (apc ? kGru8Smem : kLstm8Smem), h->device);
-  if (n_rows == 0) return LSPG_OK;
   DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  float* w = static_cast<float*>(ws);
   const int G = h->G, H = h->H;
+  if (state && step0 == 0) CUDA_TRY(cudaMemsetAsync(state, 0, sizeof(float) * static_cast<size_t>(h->L) * 2 * H, st));
+  if (n_rows == 0) return LSPG_OK;
+  float* w = static_cast<float*>(ws);
   auto P = [&](int i) { return static_cast<const float*>(h->d_packed[i]); };
   auto layer = [&](int l, const float* x, int T, float* xproj, float* dst, const float* resid) -> int {
     gemm(x, P(4 * l), h->d_ones, P(4 * l + 1), xproj, T, G * H, h->in_w[l], 0, st);
-    RecParams p{xproj, P(4 * l + 2), G == 3 ? P(4 * l + 3) : nullptr, resid, dst, T};
+    RecParams p{xproj, P(4 * l + 2), G == 3 ? P(4 * l + 3) : nullptr, resid, dst,
+                state ? state + static_cast<size_t>(l) * 2 * H : nullptr, T};
     return launch_rnn(h, cl, p, st);
   };
   int r;
@@ -462,23 +495,38 @@ int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* w
       x = dst;
     }
   } else {
-    const int D = c.input_dim, ff = c.frame_future, nframe = n_rows / 2, Ls = nframe + ff;
+    // Whole clip: the LSTM runs nframe + frame_future steps, the last frame_future over copies of the last row, which the
+    // downsample GEMM reads by clamping.  A chunk runs one step per pair it is given (every pair whole: nothing clamps).
+    const int D = c.input_dim, ff = c.frame_future, np = n_rows / 2, Ls = state ? np : np + ff;
+    // fc runs on the global steps >= frame_future (models/audio2feature_model.py:147 drops the first frame_future)
+    const int skip = state ? static_cast<int>(std::min<int64_t>(np, std::max<int64_t>(0, ff - step0))) : ff;
+    const int n_out = Ls - skip;
     float *m0 = w + off[0], *m1 = w + off[1], *xproj = w + off[2], *la = w + off[3], *lb = w + off[4];
-    // downsample over the pairs of APC rows, with the frame_future copies of the last row read by clamping
     gemm_nt_kernel<false, true><<<dim3(D / 64, (Ls + 63) / 64), 256, 0, st>>>(in, P(12), P(13), P(14), m0, Ls, D, 2 * D, 1, n_rows);
     gemm(m0, P(15), P(16), P(17), m1, Ls, D, D, 0, st);
     if ((r = layer(0, m1, Ls, xproj, la, nullptr))) return r;
     if ((r = layer(1, la, Ls, xproj, lb, nullptr))) return r;
     if ((r = layer(2, lb, Ls, xproj, la, nullptr))) return r;
-    // fc on the frames that are kept (models/audio2feature_model.py:147 drops the first frame_future)
-    const float* kept = la + static_cast<size_t>(ff) * kLstmH;
-    gemm(kept, P(18), P(19), P(20), m0, nframe, kFcW, kLstmH, 1, st);
-    gemm(m0, P(21), P(22), P(23), m1, nframe, kFcW, kFcW, 1, st);
-    gemm_nt_kernel<true, false><<<dim3((c.out_dim + 63) / 64, (nframe + 63) / 64), 256, 0, st>>>(m1, P(24), P(25), P(26), out,
-                                                                                               nframe, c.out_dim, kFcW, 0, 0);
+    if (n_out > 0) {
+      const float* kept = la + static_cast<size_t>(skip) * kLstmH;
+      gemm(kept, P(18), P(19), P(20), m0, n_out, kFcW, kLstmH, 1, st);
+      gemm(m0, P(21), P(22), P(23), m1, n_out, kFcW, kFcW, 1, st);
+      gemm_nt_kernel<true, false><<<dim3((c.out_dim + 63) / 64, (n_out + 63) / 64), 256, 0, st>>>(m1, P(24), P(25), P(26), out,
+                                                                                                 n_out, c.out_dim, kFcW, 0, 0);
+    }
   }
   CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
+}
+
+int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* ws, size_t ws_bytes, int cluster, void* stream) {
+  return forward(h, in, n_rows, 0, out, nullptr, ws, ws_bytes, cluster, stream, "lspr_forward");
+}
+
+int lspr_forward_stream(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
+                        size_t ws_bytes, int cluster, void* stream) {
+  if (h && !state) return fail(LSPG_EINVAL, "null state");
+  return forward(h, in, n_rows, step0, out, state, ws, ws_bytes, cluster, stream, "lspr_forward_stream");
 }
 
 }  // extern "C"

@@ -88,12 +88,103 @@ class HeadposeGenerator(_lib.Handle):
         for t in (a, pre, nz):
             if t.data_ptr() % 16:
                 raise ValueError("device buffers must be 16-byte aligned")
-        with self.stream() as stream:
+        with self.cuda_stream() as stream:
             self.call("generate", a.data_ptr(), n_audio, pre.data_ptr(), nz.data_ptr(), un.data_ptr() if un is not None else None,
                       float(sigma_scale), pred.data_ptr(), params.data_ptr() if params is not None else None, int(cluster),
                       stream)
         self._keep = (a, pre, nz, un)            # inputs stay alive until the caller synchronises on the result
         return (pred, params) if return_params else pred
+
+
+    def stream(self, pre_headpose=None, sigma_scale: float = 0.3, noise=None, return_params: bool = False,
+               cluster: int = 0) -> "HeadposeStream":
+        """A stream over one clip's audio rows: ``push(rows)`` returns the frames whose look-ahead is in (frame i needs
+        rows up to i + frame_future).  The concatenation equals ``generate`` of all the rows, bit for bit, given the same
+        draws.  ``pre_headpose`` defaults to zeros (demo.py:211).  ``noise``: None draws each frame's ``Sample_GMM``
+        values from torch's global CPU generator when the frame is produced, in ``draw_reference_noise``'s order (one
+        mixture component only); or a callable ``noise(first_frame, n_frames)`` returning the draws of those frames,
+        ``[n, ndim]`` or ``([n, ndim], uniform [n])``."""
+        return HeadposeStream(self, pre_headpose, sigma_scale, noise, return_params, cluster)
+
+
+class HeadposeStream:
+    """The Audio2Headpose loop over a clip pushed in pieces (``HeadposeGenerator.stream``).  Keeps on the device the
+    history ring and last sample (include/lsph.h, ``lsph_state_bytes``) and the audio rows not consumed yet - before the
+    first frame, at most ``frame_future`` of them; afterwards none - and a workspace sized for the largest push so far.
+    Pushes make no host synchronisation and, as they reuse the workspace, go on one CUDA stream."""
+
+    def __init__(self, gen: HeadposeGenerator, pre_headpose, sigma_scale: float, noise, return_params: bool, cluster: int):
+        if gen.device is None:
+            raise RuntimeError("host-only handle: created with device=-1")
+        cfg = gen.cfg
+        if cfg.loss_gmm and noise is None and cfg.ncenter > 1:
+            raise ValueError("with more than one mixture component the reference draws the component after the loop; "
+                             "pass a noise callable that returns (noise, uniform)")
+        self._gen, self._sigma, self._noise, self._params, self._cluster = gen, float(sigma_scale), noise, return_params, int(cluster)
+        pre = torch.zeros(cfg.input_ch) if pre_headpose is None else pre_headpose
+        self._pre = _lib.to_device(pre, gen.device).reshape(-1)
+        if self._pre.numel() != cfg.input_ch:
+            raise ValueError(f"pre_headpose must have {cfg.input_ch} values")
+        need = C.c_size_t()
+        gen.call("state_bytes", C.byref(need))
+        self._state = torch.empty(need.value // 4, dtype=torch.float32, device=gen.device)
+        self._ws = None                        # workspace of the hoisted GEMMs, kept across pushes
+        self._rows = torch.empty((0, 2 * cfg.apc_hidden), dtype=torch.float32, device=gen.device)
+        self._row0 = 0                         # global index of self._rows[0]
+        self.rows = 0                          # audio rows pushed so far
+        self.frames = 0                        # frames returned so far
+
+    def _draws(self, n: int):
+        cfg = self._gen.cfg
+        if not cfg.loss_gmm:
+            return None, None
+        if self._noise is None:
+            noise, _ = draw_reference_noise(n, cfg.ndim, 1)
+            uniform = None
+        else:
+            got = self._noise(self.frames, n)
+            noise, uniform = got if isinstance(got, tuple) else (got, None)
+        dev = self._gen.device
+        noise = _lib.to_device(noise, dev).reshape(n, cfg.ndim)
+        uniform = _lib.to_device(uniform, dev).reshape(n) if uniform is not None else None
+        return noise, uniform
+
+    def push(self, audio_rows):
+        """Audio rows [n, 2*APC_hidden] (any n >= 0) -> the new frames: pred [m, ndim] CUDA fp32 (and the network outputs
+        [m, out_ch] with ``return_params``), frames ``frames - m .. frames - 1``."""
+        cfg, dev = self._gen.cfg, self._gen.device
+        a = _lib.to_device(audio_rows, dev).reshape(-1, 2 * cfg.apc_hidden)
+        self.rows += a.shape[0]
+        rows = torch.cat([self._rows, a]) if self._rows.shape[0] else a
+        if rows.data_ptr() % 16:
+            rows = rows.clone()
+        n = max(0, self.rows - cfg.frame_future) - self.frames
+        pred = torch.empty((n, cfg.ndim), dtype=torch.float32, device=dev)
+        params = torch.empty((n, self._gen.out_channels), dtype=torch.float32, device=dev) if self._params else None
+        if n:
+            noise, uniform = self._draws(n)
+            need = C.c_size_t()
+            self._gen.call("stream_workspace_bytes", rows.shape[0], C.byref(need))
+            ws = self._ws = _lib.reserve(self._ws, need.value, dev)
+            with self._gen.cuda_stream() as stream:
+                self._gen.call("generate_stream", rows.data_ptr(), self._row0, rows.shape[0], self.frames, n,
+                               self._pre.data_ptr(), noise.data_ptr() if noise is not None else None,
+                               uniform.data_ptr() if uniform is not None else None, self._sigma, pred.data_ptr(),
+                               params.data_ptr() if params is not None else None, self._state.data_ptr(), ws.data_ptr(),
+                               ws.numel(), self._cluster, stream)
+            self._keep = (rows, noise, uniform)
+            self.frames += n
+        keep = self.frames + cfg.frame_future if self.frames else 0          # the first row a later frame reads
+        drop = min(max(keep - self._row0, 0), rows.shape[0])
+        self._rows = rows[drop:].clone()
+        self._row0 += drop
+        return (pred, params) if self._params else pred
+
+    def finish(self):
+        """Nothing is held back (the loop has no end padding): empty outputs."""
+        pred = torch.empty((0, self._gen.cfg.ndim), dtype=torch.float32, device=self._gen.device)
+        params = torch.empty((0, self._gen.out_channels), dtype=torch.float32, device=self._gen.device)
+        return (pred, params) if self._params else pred
 
 
 def draw_reference_noise(nframe: int, ndim: int, ncenter: int):

@@ -165,7 +165,7 @@ class LandmarkPostprocessor(_lib.Handle):
         pose = torch.empty((n, 6), **f32) if return_intermediates else None
         ws = self.workspace(n_feat, n_head)
         ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None    # noqa: E731
-        with self.stream() as stream:
+        with self.cuda_stream() as stream:
             self.call("run", ptr(feat), n_feat, ptr(head), n_head, head.shape[1], C.byref(native), ptr(lm), ptr(sh), ptr(pts),
                       ptr(pose), ws.data_ptr(), ws.numel(), stream)
         return (lm, sh, pts, pose) if return_intermediates else (lm, sh)

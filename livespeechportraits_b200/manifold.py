@@ -49,17 +49,19 @@ class ManifoldProjector(_lib.Handle):
             f = f.clone()
         return f
 
-    def knn(self, feats, k: int) -> torch.Tensor:
+    def knn(self, feats, k: int, ws: Optional[torch.Tensor] = None) -> torch.Tensor:
         """``KNN_with_torch`` on the device: int64 [n, k], ascending in ``|q|^2 + |d|^2 - 2 q.d`` (fp32), ties to the
-        lower row.  1 <= k <= min(32, N)."""
+        lower row.  1 <= k <= min(32, N).  ``ws``: a uint8 device buffer of at least ``workspace_bytes(n, k)`` bytes to
+        use instead of a new one."""
         f = self._feats(feats)
         n = f.shape[0]
         k = int(k)
         if not 1 <= k <= min(MAX_K, self.n_rows):
             raise ValueError(f"k must be in [1, {min(MAX_K, self.n_rows)}] (got {k})")
-        ws = self.workspace(n, k)
+        if ws is None or ws.numel() < self.workspace_bytes(n, k):
+            ws = self.workspace(n, k)
         ind = torch.empty((n, k), dtype=torch.int64, device=self.device)
-        with self.stream() as stream:
+        with self.cuda_stream() as stream:
             self.call("knn", f.data_ptr(), n, k, ind.data_ptr(), None, ws.data_ptr(), ws.numel(), stream)
         return ind
 
@@ -79,16 +81,16 @@ class ManifoldProjector(_lib.Handle):
         fuse = torch.empty((n, self.dim), dtype=torch.float32, device=self.device)
         blend = torch.empty((n, self.dim), dtype=torch.float32, device=self.device)
         status = torch.empty((n,), dtype=torch.int32, device=self.device)
-        with self.stream() as stream:
+        with self.cuda_stream() as stream:
             self.call("project", f.data_ptr(), n, ix.data_ptr(), k, float(percent), w.data_ptr(), fuse.data_ptr(),
                       blend.data_ptr(), status.data_ptr(), stream)
         return w, fuse, blend, status
 
-    def project_features(self, feats, k: int, percent: float = 1.0) -> torch.Tensor:
+    def project_features(self, feats, k: int, percent: float = 1.0, ws: Optional[torch.Tensor] = None) -> torch.Tensor:
         """Stage 2 of demo.py (:196-200) in one call: the blended features [n, dim] fp32 on the device.  Rows whose system
-        is singular come back as NaN (``project`` reports which)."""
+        is singular come back as NaN (``project`` reports which).  ``ws``: as for ``knn``."""
         f = self._feats(feats)
-        ind = self.knn(f, k)
+        ind = self.knn(f, k, ws)
         return self.project(f, ind, percent)[2]
 
 

@@ -46,7 +46,7 @@ class _Recurrent(_lib.Handle):
         self.call("debug_packed", which, out.ctypes.data, C.byref(n))
         return out
 
-    def _run(self, x: torch.Tensor, width: int, out_shape, cluster: int) -> torch.Tensor:
+    def _input(self, x: torch.Tensor, width: int) -> torch.Tensor:
         if not isinstance(x, torch.Tensor) or not x.is_cuda:
             raise RuntimeError("input must be a CUDA tensor (there is no CPU path)")
         if self.device is None:
@@ -54,15 +54,36 @@ class _Recurrent(_lib.Handle):
         if x.dim() != 2 or x.shape[1] != width:
             raise ValueError(f"input must be [n, {width}], got {tuple(x.shape)}")
         x = x.to(device=self.device, dtype=torch.float32).contiguous()
-        if x.data_ptr() % 16:
-            x = x.clone()
+        return x.clone() if x.data_ptr() % 16 else x
+
+    def _run(self, x: torch.Tensor, width: int, out_shape, cluster: int) -> torch.Tensor:
+        x = self._input(x, width)
         n = x.shape[0]
         out = torch.empty(out_shape, dtype=torch.float32, device=self.device)
         ws = self.workspace(n)
-        with self.stream() as stream:
+        with self.cuda_stream() as stream:
             self.call("forward", x.data_ptr(), n, out.data_ptr(), ws.data_ptr(), ws.numel(), int(cluster), stream)
         self._keep = (x, ws)           # inputs stay alive until the caller synchronises on the result
         return out
+
+    def _new_state(self) -> torch.Tensor:
+        if self.device is None:
+            raise RuntimeError("host-only handle: created with device=-1")
+        need = C.c_size_t()
+        self.call("state_bytes", C.byref(need))
+        return torch.zeros(need.value // 4, dtype=torch.float32, device=self.device)
+
+    def _run_stream(self, x: torch.Tensor, step0: int, state: torch.Tensor, ws, n_out: int, out_dim: int, cluster: int):
+        """One ``lspr_forward_stream`` call: ``x`` [n, width] from global step ``step0``, with the stream's workspace
+        ``ws`` (grown if too small); returns ([n_out, out_dim], the workspace)."""
+        n = x.shape[0]
+        out = torch.empty((n_out, out_dim), dtype=torch.float32, device=self.device)
+        ws = _lib.reserve(ws, self.workspace_bytes(n), self.device)
+        with self.cuda_stream() as stream:
+            self.call("forward_stream", x.data_ptr() if n else None, n, int(step0), out.data_ptr() if n_out else None,
+                      state.data_ptr(), ws.data_ptr(), ws.numel(), int(cluster), stream)
+        self._keep = x
+        return out, ws
 
 
 class ApcEncoder(_Recurrent):
@@ -93,6 +114,35 @@ class ApcEncoder(_Recurrent):
         return self._run(mel, self.mel_dim, (mel.shape[0], self.hidden), cluster)
 
     __call__ = forward
+
+    def stream(self, cluster: int = 0) -> "ApcStream":
+        """A stream over one clip's mel frames: ``push(mel)`` returns the features of the rows pushed, and the
+        concatenation equals ``forward`` of all of them, bit for bit."""
+        return ApcStream(self, cluster)
+
+
+class ApcStream:
+    """The APC encoder over a clip pushed in pieces (``ApcEncoder.stream``).  Keeps each layer's last h and a workspace
+    sized for the largest push so far on the device; every push is enqueued on the current stream with no host
+    synchronisation (the pushes of one stream reuse the workspace, so they go on one CUDA stream)."""
+
+    def __init__(self, enc: ApcEncoder, cluster: int = 0):
+        self._enc, self._cluster = enc, int(cluster)
+        self._state = enc._new_state()
+        self._ws = None                        # workspace, kept across pushes
+        self.rows = 0                          # mel frames pushed so far
+
+    def push(self, mel: torch.Tensor) -> torch.Tensor:
+        """mel [n, mel_dim] CUDA (n >= 0) -> features [n, hidden] CUDA fp32."""
+        x = self._enc._input(mel, self._enc.mel_dim)
+        out, self._ws = self._enc._run_stream(x, self.rows, self._state, self._ws, x.shape[0], self._enc.hidden,
+                                              self._cluster)
+        self.rows += x.shape[0]
+        return out
+
+    def finish(self) -> torch.Tensor:
+        """Nothing is held back: an empty [0, hidden] tensor."""
+        return torch.empty((0, self._enc.hidden), dtype=torch.float32, device=self._enc.device)
 
 
 def mouth_output_size(opt) -> int:
@@ -128,6 +178,63 @@ class MouthGenerator(_Recurrent):
         if n < 2:
             raise ValueError("need at least 2 APC rows")
         return self._run(feats, self.apc_hidden, (n // 2, self.out_dim), 0)
+
+    def stream(self) -> "MouthStream":
+        """A stream over one clip's APC features: ``push(feats)`` returns the track rows whose inputs are all in (frame f
+        needs APC rows up to 2 (f + frame_future) + 1), ``finish()`` the last ``frame_future`` rows, built from copies of
+        the last APC row.  The concatenation equals ``generate`` of all the rows, bit for bit."""
+        return MouthStream(self)
+
+
+class MouthStream:
+    """Audio2Mouth over a clip pushed in pieces (``MouthGenerator.stream``).  Keeps the LSTM's h and c, one pending odd
+    APC row, the last APC row and a workspace sized for the largest push so far on the device; every call is enqueued on
+    the current stream with no host synchronisation (one CUDA stream per stream object, as the workspace is reused)."""
+
+    def __init__(self, gen: MouthGenerator):
+        self._gen = gen
+        self._state = gen._new_state()
+        self._ws = None                        # workspace, kept across pushes
+        self._odd = None                       # an APC row waiting for its pair
+        self._last = None                      # the last APC row: finish() pads with copies of it
+        self.pairs = 0                         # LSTM steps run so far
+        self.frames = 0                        # track rows returned so far
+        self.finished = False
+
+    def _run(self, x: torch.Tensor) -> torch.Tensor:
+        ff, np_ = self._gen.frame_future, x.shape[0] // 2
+        n_out = max(0, self.pairs + np_ - max(self.pairs, ff))          # the new global steps >= frame_future
+        out, self._ws = self._gen._run_stream(x, self.pairs, self._state, self._ws, n_out, self._gen.out_dim, 0)
+        self.pairs += np_
+        self.frames += n_out
+        return out
+
+    def push(self, feats: torch.Tensor) -> torch.Tensor:
+        """APC features [n, APC_hidden] CUDA (any n >= 0) -> the new track rows [m, out_dim], frames
+        ``frames - m .. frames - 1``."""
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        x = self._gen._input(feats, self._gen.apc_hidden)
+        if x.shape[0]:
+            self._last = x[-1:].clone()
+        if self._odd is not None:
+            x = torch.cat([self._odd, x])
+        even = x.shape[0] // 2 * 2
+        self._odd = x[even:].clone() if even < x.shape[0] else None
+        return self._run(x[:even])
+
+    def finish(self) -> torch.Tensor:
+        """The last ``frame_future`` track rows (fewer if the clip had fewer pairs; none for an empty clip)."""
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        self.finished = True
+        if self._odd is not None:
+            n = 2 * self.pairs + 1
+            raise RuntimeError(f"shape '[1, -1, {2 * self._gen.apc_hidden}]' is invalid for input of size "
+                               f"{(n + 2 * self._gen.frame_future) * self._gen.apc_hidden}")
+        if self.pairs == 0 or self._gen.frame_future == 0:
+            return torch.empty((0, self._gen.out_dim), dtype=torch.float32, device=self._gen.device)
+        return self._run(self._last.expand(2 * self._gen.frame_future, -1).contiguous())
 
 
 # ------------------------------------------------------------------------------------------------------------------
