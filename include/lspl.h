@@ -77,6 +77,38 @@ int lspl_run(lspl_handle h, const float* pred_feat, int n_feat, const float* pre
              const lspl_params* p, float* landmarks, float* shoulders, float* final_pts3d, float* pred_headpose,
              void* workspace, size_t workspace_bytes, void* stream);
 
+/* Streaming: the same frames from track rows that arrive in pieces (the live path of livespeechportraits_b200/stream.py).
+ *
+ * Frame t of a call equals frame t of lspl_run on the whole tracks, value for value, except the outer lips of crossed
+ * frames (below).  Row i of the mouth track is feat[i - feat_row0] (n_feat_rows rows given), row i of the head track
+ * head[(i - head_row0) * head_stride]; frames frame0 .. frame0 + n_frames - 1 are written to row 0 .. n_frames - 1 of
+ * the outputs.  The mouth reflects at nframe_total (= min(n_feat, n_head) of the whole clip), the head at
+ * n_head_total, as in lspl_run; each total is -1 while the clip goes on.  The eyebrow candidate is t % m with the
+ * global t.
+ *
+ * Refused with LSPG_EINVAL: a frame at or past a known total; while nframe_total is -1, a frame t with
+ * t + rm >= head_row0 + n_head_rows (the mouth window must be interior: nframe may yet end at the head rows); a row
+ * window not covered, i.e. the mouth rows max(0, t - rm) .. t + rm and the head rows max(0, t - rh) .. t + rh
+ * (rh = max(rr, rt); capped at a known total minus one) must lie in the rows given for every frame emitted.  Rows
+ * and frames end at or below 2^29.
+ *
+ * The live lip fix.  A frame is crossed when all three lower inner-lip y exceed the upper ones (as in lspl_run); its
+ * inner lips move by its own half-differences (as in lspl_run).  Its outer lips move by the running mean of
+ * half_inner_y_diff over the crossed frames up to and including it: S += h_t, C += 1, shift_t = S / (3 C), with h_t
+ * the three-term fp64 sum lspl_run adds up, taken one frame at a time in frame order.  The result does not depend on
+ * how the clip was cut into calls; at the last crossed frame the shift equals lspl_run's clip mean up to fp64
+ * summation order.  `state` (lspl_stream_state_bytes, device memory) carries S and C between calls; frame0 == 0 starts
+ * them from zero.
+ *
+ * At most three launches on `stream`; allocates nothing, does not synchronise the host, no atomics: identical inputs
+ * give bit-identical outputs.  Host-only handles check the arguments and return LSPG_ENODEV. */
+int lspl_stream_state_bytes(lspl_handle h, size_t* out);
+int lspl_stream_workspace_bytes(lspl_handle h, int n_frames, size_t* out);
+int lspl_run_stream(lspl_handle h, const float* feat, int feat_row0, int n_feat_rows, const float* head, int head_row0,
+                    int n_head_rows, int head_stride, int frame0, int n_frames, int nframe_total, int n_head_total,
+                    const lspl_params* p, float* landmarks, float* shoulders, float* final_pts3d, float* pred_headpose,
+                    void* state, void* workspace, size_t workspace_bytes, void* stream);
+
 int lspl_destroy(lspl_handle h);
 const char* lspl_last_error(void);
 

@@ -124,6 +124,9 @@ ARGTYPES = {
     "lspl_load_identity": [_p, C.POINTER(LsplIdentity)],
     "lspl_workspace_bytes": [_p, _i, _i, _psz],
     "lspl_run": [_p, _p, _i, _p, _i, _i, C.POINTER(LsplParams), _p, _p, _p, _p, _p, _sz, _p],
+    "lspl_stream_state_bytes": [_p, _psz],
+    "lspl_stream_workspace_bytes": [_p, _i, _psz],
+    "lspl_run_stream": [_p, _p, _i, _i, _p, _i, _i, _i, _i, _i, _i, _i, C.POINTER(LsplParams), _p, _p, _p, _p, _p, _p, _sz, _p],
     "lspl_destroy": [_p],
     "lspl_last_error": [],
     # include/lspr.h (APC encoder GRU and Audio2Mouth LSTM, demo.py stages 1 and 3)

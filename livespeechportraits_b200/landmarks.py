@@ -6,13 +6,14 @@ and projects every frame in two Python loops (``project_landmarks`` for the 73 f
 points).  ``LandmarkPostprocessor.run`` does all of it in two kernels (include/lspl.h, csrc/lspl.cu) and leaves
 ``pred_landmarks`` / ``pred_shoulders`` on the device, where ``Feature2Face_G.draw_feature_maps`` and
 ``ClipRenderer.render_clip_from_landmarks`` take them.  ``postprocess_clip`` is the numpy-in, numpy-out form with
-demo.py's variable names.  There is no CPU path.
+demo.py's variable names.  ``LandmarkPostprocessor.stream`` opens a ``LandmarkStream``: track rows pushed as they
+arrive from ``stream.AudioStream``, landmarks out as soon as the smoothing windows are in.  There is no CPU path.
 """
 from __future__ import annotations
 
 import ctypes as C
 from dataclasses import dataclass
-from typing import Optional, Sequence
+from typing import NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
@@ -111,6 +112,23 @@ def _native_params(p: StageParams, image_pad) -> _lib.LsplParams:
     return n
 
 
+def radii(params: StageParams) -> Tuple[int, int]:
+    """The look-ahead of stage 5 in frames: the mouth smoothing radius ``rm`` (0 without smoothing) and
+    ``rh = max(rr, rt)`` of the two head-pose smoothings, each ``int(4 sigma + 0.5)``."""
+    r = lambda s: int(4.0 * float(s) + 0.5)                       # noqa: E731
+    rm = r(params.feat_smooth_sigma) if float(params.feat_smooth_sigma) > 0 else 0
+    return rm, max(r(s) for s in params.head_smooth_sigma)
+
+
+class LandmarkRows(NamedTuple):
+    """What one ``LandmarkStream.push`` or ``finish`` returned: frames ``frame0 .. frame0 + k - 1``."""
+    landmarks: torch.Tensor                        # [k, 73, 2]
+    shoulders: torch.Tensor                        # [k, 18, 2]
+    frame0: int
+    final_pts3d: Optional[torch.Tensor] = None     # [k, 73, 3] with return_intermediates
+    pred_headpose: Optional[torch.Tensor] = None   # [k, 6] with return_intermediates
+
+
 class LandmarkPostprocessor(_lib.Handle):
     """Owns the native handle and the device copy of one identity's constants (taken at construction)."""
     prefix, what = "lspl", "the landmark post-processing"
@@ -169,6 +187,109 @@ class LandmarkPostprocessor(_lib.Handle):
             self.call("run", ptr(feat), n_feat, ptr(head), n_head, head.shape[1], C.byref(native), ptr(lm), ptr(sh), ptr(pts),
                       ptr(pose), ws.data_ptr(), ws.numel(), stream)
         return (lm, sh, pts, pose) if return_intermediates else (lm, sh)
+
+    def stream(self, params: StageParams, image_pad: Optional[Sequence[int]] = None,
+               return_intermediates: bool = False) -> "LandmarkStream":
+        """A stream over one clip's mouth and head-pose track rows (``LandmarkStream``)."""
+        return LandmarkStream(self, params, image_pad, return_intermediates)
+
+    def stream_state(self) -> torch.Tensor:
+        """A device buffer for ``lspl_run_stream``'s lip-fix state (its first call, at frame 0, initialises it)."""
+        if self.device is None:
+            raise RuntimeError("host-only handle: created with device=-1")
+        need = C.c_size_t()
+        self.call("stream_state_bytes", C.byref(need))
+        return torch.empty(need.value, dtype=torch.uint8, device=self.device)
+
+    def device_rows(self, rows, width: int) -> torch.Tensor:
+        """Track rows (numpy or torch, any device) as contiguous fp32 device rows of their first ``width`` columns:
+        ``[n, 75]`` (or ``[n, 25, 3]``) for the mouth, ``[n, >= 6]`` for the head pose (``width`` 6)."""
+        t = _lib.to_device(rows, self.device)
+        t = t.reshape(-1, 75) if width == 75 and t.dim() == 3 else t
+        if t.dim() != 2 or t.shape[1] < width or (width == 75 and t.shape[1] != 75):
+            raise ValueError(f"track rows must be [n, {width if width == 75 else '>= 6'}], got {tuple(t.shape)}")
+        return t[:, :width].contiguous()
+
+    def run_stream(self, feat, feat_row0: int, head, head_row0: int, frame0: int, n: int, nframe_total: int,
+                   n_head_total: int, native, state, ws, return_intermediates: bool):
+        """One ``lspl_run_stream`` call over the device rows ``feat`` [*, 75] and ``head`` [*, 6] (fp32, contiguous):
+        returns ``LandmarkRows`` of frames ``frame0 .. frame0 + n - 1`` and the workspace used (``ws`` or a larger one)."""
+        dev = self.device
+        f32 = dict(dtype=torch.float32, device=dev)
+        lm, sh = torch.empty((n, N_PTS, 2), **f32), torch.empty((n, N_SHOULDERS, 2), **f32)
+        pts = torch.empty((n, N_PTS, 3), **f32) if return_intermediates else None
+        pose = torch.empty((n, 6), **f32) if return_intermediates else None
+        need = C.c_size_t()
+        self.call("stream_workspace_bytes", n, C.byref(need))
+        ws = _lib.reserve(ws, need.value, dev)
+        ptr = lambda t: t.data_ptr() if t is not None and t.numel() else None    # noqa: E731
+        with self.cuda_stream() as stream:
+            self.call("run_stream", ptr(feat), feat_row0, feat.shape[0], ptr(head), head_row0, head.shape[0], 6, frame0, n,
+                      nframe_total, n_head_total, C.byref(native), ptr(lm), ptr(sh), ptr(pts), ptr(pose), state.data_ptr(),
+                      ws.data_ptr(), ws.numel(), stream)
+        return LandmarkRows(lm, sh, frame0, pts, pose), ws
+
+
+class LandmarkStream:
+    """Stage 5 over track rows that arrive in pieces (``LandmarkPostprocessor.stream``).  ``push(mouth_rows, head_rows)``
+    takes the new rows of the Audio2Mouth track ([m, 75] or [m, 25, 3]) and of the head-pose track ([h, >= 6]), in any
+    counts, and ``finish()`` ends the clip; both return ``LandmarkRows`` of the frames that became ready
+    (``stream.landmark_counts``: frame t needs mouth rows up to t + rm and head rows up to t + rh; at the end every
+    frame of ``nframe = min(n_feat, n_head)``).
+
+    Every value equals ``run`` on the whole tracks bit for bit, except the outer lips of crossed frames: there
+    ``solve_intersect_mouth``'s mean over all crossed frames of the clip, which a live stream cannot know, becomes the
+    running mean over the crossed frames up to and including the frame (include/lspl.h, ``lspl_run_stream``).  It does
+    not depend on how the rows were cut into pushes, and at the clip's last crossed frame it equals the clip mean up to
+    fp64 summation order.
+
+    Kept on the device: the mouth rows from ``frames - rm``, the head rows from ``frames - rh``, the lip-fix state (a
+    running sum and count) and a workspace sized for the largest push so far.  Pushes make no host synchronisation and
+    go on one CUDA stream."""
+
+    def __init__(self, post, params: StageParams, image_pad=None, return_intermediates: bool = False):
+        self._post = post
+        self._native = _native_params(params, image_pad)
+        self.rm, self.rh = radii(params)
+        self._inter = bool(return_intermediates)
+        self._state = post.stream_state()
+        self._ws = None
+        self._feat = post.device_rows(torch.empty((0, 75)), 75)
+        self._head = post.device_rows(torch.empty((0, 6)), 6)
+        self._feat_row0 = self._head_row0 = 0      # global index of the first kept row
+        self.feat_rows = self.head_rows = 0        # rows pushed so far
+        self.frames = 0                            # frames returned so far
+        self.finished = False
+
+    def push(self, mouth_rows, head_rows) -> LandmarkRows:
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        feat, head = self._post.device_rows(mouth_rows, 75), self._post.device_rows(head_rows, 6)
+        self._feat = torch.cat([self._feat, feat]) if feat.shape[0] else self._feat
+        self._head = torch.cat([self._head, head]) if head.shape[0] else self._head
+        self.feat_rows += feat.shape[0]
+        self.head_rows += head.shape[0]
+        return self._emit(False)
+
+    def finish(self) -> LandmarkRows:
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        self.finished = True
+        return self._emit(True)
+
+    def _emit(self, finished: bool) -> LandmarkRows:
+        from .stream import landmark_counts
+        n = landmark_counts(self.feat_rows, self.head_rows, finished, self.rm, self.rh) - self.frames
+        nframe, n_head = (min(self.feat_rows, self.head_rows), self.head_rows) if finished else (-1, -1)
+        out, self._ws = self._post.run_stream(self._feat, self._feat_row0, self._head, self._head_row0, self.frames, n,
+                                              nframe, n_head, self._native, self._state, self._ws, self._inter)
+        self.frames += n
+        # keep the rows later frames read: mouth from frames - rm, head from frames - rh
+        drop = min(max(self.frames - self.rm - self._feat_row0, 0), self._feat.shape[0])
+        self._feat, self._feat_row0 = self._feat[drop:].clone(), self._feat_row0 + drop
+        drop = min(max(self.frames - self.rh - self._head_row0, 0), self._head.shape[0])
+        self._head, self._head_row0 = self._head[drop:].clone(), self._head_row0 + drop
+        return out if self._inter else LandmarkRows(out.landmarks, out.shoulders, out.frame0)
 
 
 def postprocess_clip(pred_Feat, pred_Head, mean_pts3d, std_mean_pts3d, candidate_eye_brow, mean_translation, ref_trans,

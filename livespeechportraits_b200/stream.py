@@ -9,6 +9,10 @@ never waits for the device.
 
 The look-ahead is the models': Audio2Mouth's ``frame_future`` (18) and Audio2Headpose's (15) video frames, i.e. about
 0.32 s and 0.27 s of audio at 60 fps, plus the mel window itself.
+
+``PortraitStream`` goes on to frames: the track rows through stage 5 (``LandmarkPostprocessor.stream``, which adds the
+smoothing radii to the look-ahead: frame t needs head-pose row t + max(rr, rt), so for May's settings APC pair t + 55),
+then the rasteriser and the generator, one frame per generator call.
 """
 from __future__ import annotations
 
@@ -55,6 +59,24 @@ def ready_counts(n_samples: int, finished: bool, frame_len: int = 266, step: flo
     pairs = mel // 2
     mouth = pairs if finished else max(0, pairs - mouth_future)
     return Counts(mel, mel, mouth, max(0, pairs - headpose_future))
+
+
+def landmark_counts(n_feat: int, n_head: int, finished: bool, rm: int, rh: int) -> int:
+    """Stage-5 frames ready from ``n_feat`` mouth and ``n_head`` head-pose track rows: frame t needs mouth rows up to
+    t + rm (and t + rm < n_head, since the mouth reflects at nframe = min(n_feat, n_head)) and head rows up to t + rh;
+    at the end of the clip all ``min(n_feat, n_head)`` frames."""
+    if finished:
+        return min(n_feat, n_head)
+    return max(0, min(min(n_feat, n_head) - rm, n_head - rh))
+
+
+def portrait_counts(n_samples: int, finished: bool, params, frame_len: int = 266, step: float = SR * 0.5 / FPS,
+                    mouth_future: int = 18, headpose_future: int = 15) -> int:
+    """Portrait frames ready after ``n_samples`` samples: ``landmark_counts`` of the track rows ``ready_counts`` gives,
+    with the radii of ``params`` (``landmarks.StageParams``)."""
+    from .landmarks import radii
+    c = ready_counts(n_samples, finished, frame_len, step, mouth_future, headpose_future)
+    return landmark_counts(c.mouth, c.headpose, finished, *radii(params))
 
 
 @dataclasses.dataclass
@@ -126,4 +148,59 @@ class AudioStream:
         self.apc_rows += apc.shape[0]
         self.mouth_frames += mouth.shape[0]
         self.headpose_frames += head.shape[0]
+        return out
+
+
+@dataclasses.dataclass
+class PortraitFrames:
+    """What one ``PortraitStream.push`` or ``finish`` returned: frames ``frame0 .. frame0 + k - 1``."""
+    frames: torch.Tensor          # [k, H, W, 3] uint8 images (tensor2im's layout)
+    frame0: int
+    landmarks: torch.Tensor       # [k, 73, 2] the landmarks they were drawn from
+    shoulders: torch.Tensor       # [k, 18, 2]
+    rows: StreamRows              # the track rows of stages 1-4 this push produced
+
+
+class PortraitStream:
+    """Live audio to portrait frames: ``AudioStream`` (stages 1-4) -> ``LandmarkStream`` (stage 5) ->
+    ``net.draw_feature_maps`` -> ``net.render_image`` (stage 6).  ``push(samples)`` / ``finish()`` return
+    ``PortraitFrames``; how many is ``portrait_counts``.
+
+    ``audio_stream`` is a fresh ``AudioStream``; ``post`` a ``LandmarkPostprocessor``, ``params`` its ``StageParams``;
+    ``net`` the ``Feature2Face_G`` and ``cand`` its candidate images ``[1, 3 k, H, W]`` on the device.  The landmarks
+    follow ``LandmarkStream``'s live lip-fix rule.  A push's feature maps are rasterised in one call into a staging
+    buffer kept across pushes (the rasteriser is exact frame by frame); the generator then renders one frame per call,
+    so every frame goes through the same plan and the same CUDA graph and its bits do not depend on the push sizes.
+    Pushes make no host synchronisation and go on one CUDA stream."""
+
+    def __init__(self, audio_stream: AudioStream, post, params, net, cand, size=(512, 512), image_pad=None):
+        self._audio = audio_stream
+        self._lm = post.stream(params, image_pad)
+        self._net, self._cand = net, cand
+        self._size = (int(size[0]), int(size[1]))
+        self._maps = None                     # [k, 1, H, W] staging for the feature maps, kept across pushes
+        self.frames = 0
+
+    def push(self, samples) -> PortraitFrames:
+        rows = self._audio.push(samples)
+        return self._render(rows, [self._lm.push(rows.mouth, rows.headpose)])
+
+    def finish(self) -> PortraitFrames:
+        rows = self._audio.finish()
+        return self._render(rows, [self._lm.push(rows.mouth, rows.headpose), self._lm.finish()])
+
+    def _render(self, rows: StreamRows, parts) -> PortraitFrames:
+        lm = torch.cat([p.landmarks for p in parts]) if len(parts) > 1 else parts[0].landmarks
+        sh = torch.cat([p.shoulders for p in parts]) if len(parts) > 1 else parts[0].shoulders
+        k = lm.shape[0]
+        w, h = self._size
+        if self._maps is None or self._maps.shape[0] < k:
+            self._maps = torch.empty((max(k, 1), 1, h, w), dtype=torch.float32, device=lm.device)
+        frames = torch.empty((k, h, w, 3), dtype=torch.uint8, device=lm.device)
+        if k:
+            maps = self._net.draw_feature_maps(lm, sh, self._size, out=self._maps[:k])
+            for i in range(k):
+                self._net.render_image(maps[i:i + 1], self._cand, out=frames[i:i + 1])
+        out = PortraitFrames(frames, self.frames, lm, sh, rows)
+        self.frames += k
         return out
