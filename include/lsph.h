@@ -45,7 +45,7 @@ typedef struct lsph_config {
 } lsph_config;
 
 /* Replaces Audio2Headpose.__init__ (models/audio2headpose.py:8-37) + init_net's device move.  device == -1: host-only
- * handle (weight packing introspection; lsph_generate returns LSPG_ENODEV). */
+ * handle (weight packing introspection; lsph_generate_stream returns LSPG_ENODEV). */
 int lsph_create(lsph_handle* out, const lsph_config* cfg, int device);
 
 /* Replaces load_state_dict of the Audio2Headpose module (models/base_model.py:193-223): keys as in
@@ -53,19 +53,6 @@ int lsph_create(lsph_handle* out, const lsph_config* cfg, int device);
  * optional "module." prefix, host fp32.  Eval-mode BatchNorm1d is folded into the first linear layer's epilogue.
  * Every parameter must be present (LSPG_ESTATE otherwise: there is no initialiser on this side). */
 int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n);
-
-/* Replaces Audio2HeadposeModel.generate_sequences (models/audio2headpose_model.py:133-187; WaveNet decoder,
- * fill_zero=True).  All pointers are DEVICE pointers, fp32, contiguous:
- *   audio_feats  [n_audio, 2*apc_hidden]   (the reshape at :148 already applied)
- *   pre_headpose [input_ch]                (demo.py:211: zeros)
- *   noise        [n_audio - frame_future, ndim]   the torch.randn draws of Sample_GMM (losses.py:96), one row per frame
- *   uniform      [n_audio - frame_future] or NULL: one U(0,1) draw per frame selecting the mixture component when
- *                ncenter > 1 (inverse CDF of the softmax weights; torch.multinomial's own stream is not reproduced)
- *   out_pred     [n_audio - frame_future, ndim]   = pred_headpose (:186)
- *   out_params   [n_audio - frame_future, out_ch] or NULL: the network output (GMM parameters) of every frame
- * cluster: CTAs that share a frame's work (1 or 8; 0 = library default).  Asynchronous on `stream`. */
-int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
-                  const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream);
 
 /* Bytes of the state of one stream (works on a host-only handle): fp32 [L][ring][residual_ch] history ring - the input of
  * block l at absolute step t sits in slot t mod ring, ring the smallest power of two above the largest dilation (128 for
@@ -75,21 +62,29 @@ int lsph_state_bytes(lsph_handle h, size_t* bytes);
 /* Bytes of device workspace lsph_generate_stream needs for n_audio audio rows. */
 int lsph_stream_workspace_bytes(lsph_handle h, int n_audio, size_t* bytes);
 
-/* One chunk of a stream: frames frame0 .. frame0 + n_frames - 1 of the head-pose track.  Calls with consecutive frame
- * ranges starting at 0 give, concatenated, the rows lsph_generate returns for the whole clip, bit for bit: the hoisted
- * GEMMs are computed row by row and the loop runs the same steps in the same order.
- *   audio_feats  [n_audio, 2*apc_hidden]: the clip's audio rows audio_row0 .. audio_row0 + n_audio - 1.  They must cover
- *                rows frame0 + frame_future .. frame0 + n_frames - 1 + frame_future, and from row 0 when frame0 == 0
- *                (the rf - 1 warm-up steps that replay window 0 read rows 0 .. frame_future - 1).  Frame i needs audio
- *                up to row i + frame_future and nothing later.
- *   noise        [n_frames, ndim], uniform [n_frames] or NULL: the draws of frames frame0 .. (as for lsph_generate)
- *   out_pred     [n_frames, ndim], out_params [n_frames, out_ch] or NULL
+/* Replaces Audio2HeadposeModel.generate_sequences (models/audio2headpose_model.py:133-187; WaveNet decoder,
+ * fill_zero=True) on frames frame0 .. frame0 + n_frames - 1 of the head-pose track.  A clip of n_audio audio rows has
+ * n_audio - frame_future frames; the whole clip is one call with frame0 = 0, audio_row0 = 0 and
+ * n_frames = n_audio - frame_future, and calls with consecutive frame ranges starting at 0 give, concatenated, the same
+ * rows bit for bit: the hoisted GEMMs are computed row by row and the loop runs the same steps in the same order.
+ * All pointers are DEVICE pointers, fp32, contiguous:
+ *   audio_feats  [n_audio, 2*apc_hidden] (the reshape at :148 already applied): the clip's audio rows audio_row0 ..
+ *                audio_row0 + n_audio - 1.  They must cover rows frame0 + frame_future .. frame0 + n_frames - 1 +
+ *                frame_future, and from row 0 when frame0 == 0 (the rf - 1 warm-up steps that replay window 0 read rows
+ *                0 .. frame_future - 1).  Frame i needs audio up to row i + frame_future and nothing later.
+ *   pre_headpose [input_ch]                (demo.py:211: zeros)
+ *   noise        [n_frames, ndim]: the torch.randn draws of Sample_GMM (losses.py:96), one row per frame
+ *   uniform      [n_frames] or NULL: one U(0,1) draw per frame selecting the mixture component when ncenter > 1 (inverse
+ *                CDF of the softmax weights; torch.multinomial's own stream is not reproduced)
+ *   out_pred     [n_frames, ndim] = pred_headpose (:186)
+ *   out_params   [n_frames, out_ch] or NULL: the network output (GMM parameters) of every frame
  *   state        lsph_state_bytes of caller-owned device memory, 16-byte aligned.  frame0 == 0 starts the loop from
  *                pre_headpose (the ring needs no clearing: reads before step 0 are window 0's zero padding); every call
  *                leaves the state after its last frame, which the call for frame0 + n_frames continues from.
  *   ws           lsph_stream_workspace_bytes(h, n_audio) bytes, 256-byte aligned.
- * n_frames == 0 does nothing.  LSPG_EINVAL (checked before the device, so also on a host-only handle) for a null state or
- * audio rows that do not cover the frames; LSPG_ENODEV on a host-only handle.  Asynchronous on `stream`. */
+ * cluster: CTAs that share a frame's work (1 or 8; 0 = library default).  n_frames == 0 does nothing.  LSPG_EINVAL
+ * (checked before the device, so also on a host-only handle) for a null state or audio rows that do not cover the frames;
+ * LSPG_ENODEV on a host-only handle.  Asynchronous on `stream`. */
 int lsph_generate_stream(lsph_handle h, const float* audio_feats, int audio_row0, int n_audio, int frame0, int n_frames,
                          const float* pre_headpose, const float* noise, const float* uniform, float sigma_scale,
                          float* out_pred, float* out_params, float* state, void* ws, size_t ws_bytes, int cluster,

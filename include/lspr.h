@@ -44,7 +44,7 @@ typedef struct lspr_config {
                         predict_length; 75 shipped), 1..4096.  APC: ignored */
 } lspr_config;
 
-/* device == -1: host-only handle (weight packing introspection; lspr_forward returns LSPG_ENODEV). */
+/* device == -1: host-only handle (weight packing introspection; lspr_forward_stream returns LSPG_ENODEV). */
 int lspr_create(lspr_handle* out, const lspr_config* cfg, int device);
 
 /* Replaces load_state_dict.  Keys as in the reference module's state_dict(), optional "module." prefix, host fp32:
@@ -55,33 +55,29 @@ int lspr_create(lspr_handle* out, const lspr_config* cfg, int device);
  * (eps 1e-5) is folded into the preceding linear layer's epilogue as a per-channel scale and shift. */
 int lspr_load_weights(lspr_handle h, const lspg_tensor* tensors, int n);
 
-/* Bytes of device workspace lspr_forward needs for n_rows input rows. */
+/* Bytes of device workspace lspr_forward_stream needs for n_rows input rows. */
 int lspr_workspace_bytes(lspr_handle h, int n_rows, size_t* bytes);
-
-/* DEVICE pointers, fp32, contiguous, 16-byte aligned:
- *   APC    in [n_rows, input_dim] mel frames                -> out [n_rows, hidden]   (n_rows >= 0)
- *   MOUTH  in [n_rows, input_dim] APC features, n_rows even -> out [n_rows / 2, out_dim]   (n_rows >= 2)
- * ws: lspr_workspace_bytes(h, n_rows) bytes, 256-byte aligned.  cluster: CTAs per recurrence launch, 0 = library
- * choice (APC: 16 when a 16-CTA cluster can be scheduled, else 8 with part of W_hh read from L2; MOUTH: 8); APC accepts
- * 8 or 16, MOUTH 8.  Asynchronous on `stream`. */
-int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* ws, size_t ws_bytes, int cluster, void* stream);
 
 /* Bytes of the recurrent state of one stream: fp32 [num_layers][2][hidden], each layer's h and (LSTM) c.  Works on a
  * host-only handle. */
 int lspr_state_bytes(lspr_handle h, size_t* bytes);
 
-/* One chunk of a stream: the clip's input rows pushed in pieces.  The chunks' outputs, concatenated, are bit-identical to
- * lspr_forward on the whole clip, because the input projections and MLPs are computed row by row and every recurrent step
- * is the same arithmetic whether it starts a launch or not.  state: lspr_state_bytes of caller-owned device memory, 16-byte
- * aligned, carried from call to call; step0 == 0 zeroes it (h_0 = c_0 = 0) and every call replaces it with the state after
- * its last step.
- *   APC    in: rows step0 .. step0 + n_rows - 1 of the mel frames -> out [n_rows, hidden].
- *   MOUTH  in: n_rows (even, >= 0) APC rows, the pairs step0 .. step0 + n_rows/2 - 1 -> out: the track rows of the global
- *          LSTM steps max(step0, frame_future) .. step0 + n_rows/2 - 1, row s - frame_future for step s.  To end a clip of
- *          n APC rows, pass 2 * frame_future copies of its last row with step0 = n / 2: that yields its last frame_future
- *          track rows (models/audio2feature_model.py:134).
- * ws: lspr_workspace_bytes(h, n_rows) bytes, cluster as for lspr_forward.  LSPG_EINVAL for a null state or an odd MOUTH
- * row count (checked before the device, so also on a host-only handle); LSPG_ENODEV on a host-only handle. */
+/* One span of a clip: its input rows from global step step0.  A whole clip is one call with step0 = 0; a stream pushes
+ * the rows in pieces, and the pieces' outputs, concatenated, are bit-identical to that call, because the input
+ * projections and MLPs are computed row by row and every recurrent step is the same arithmetic whether it starts a launch
+ * or not.  DEVICE pointers, fp32, contiguous, 16-byte aligned.  state: lspr_state_bytes of caller-owned device memory,
+ * carried from call to call; step0 == 0 zeroes it (h_0 = c_0 = 0) and every call replaces it with the state after its
+ * last step.
+ *   APC    in: rows step0 .. step0 + n_rows - 1 of the mel frames [n_rows, input_dim] -> out [n_rows, hidden].
+ *   MOUTH  in: n_rows (even, >= 0) APC rows [n_rows, input_dim], the pairs step0 .. step0 + n_rows/2 - 1 -> out: the
+ *          track rows [.., out_dim] of the global LSTM steps max(step0, frame_future) .. step0 + n_rows/2 - 1, row
+ *          s - frame_future for step s.  A clip of n APC rows ends with 2 * frame_future copies of its last row
+ *          (models/audio2feature_model.py:134), the pairs n/2 .. n/2 + frame_future - 1: they yield its last
+ *          frame_future track rows, so the whole clip is one call on its n rows followed by those copies.
+ * ws: lspr_workspace_bytes(h, n_rows) bytes, 256-byte aligned.  cluster: CTAs per recurrence launch, 0 = library choice
+ * (APC: 16 when a 16-CTA cluster can be scheduled, else 8 with part of W_hh read from L2; MOUTH: 8); APC accepts 8 or 16,
+ * MOUTH 8.  Asynchronous on `stream`.  LSPG_EINVAL for a null state or an odd MOUTH row count (checked before the device,
+ * so also on a host-only handle); LSPG_ENODEV on a host-only handle. */
 int lspr_forward_stream(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
                         size_t ws_bytes, int cluster, void* stream);
 

@@ -3,7 +3,6 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
-import functools
 import os
 from typing import List, Optional, Tuple
 
@@ -96,7 +95,6 @@ ARGTYPES = {
     # include/lsph.h (Audio2Headpose generation loop)
     "lsph_create": [_out_handle, C.POINTER(LsphConfig), _i],
     "lsph_load_weights": [_p, _tensors, _i],
-    "lsph_generate": [_p, _p, _i, _p, _p, _p, C.c_float, _p, _p, _i, _p],
     "lsph_state_bytes": [_p, _psz],
     "lsph_stream_workspace_bytes": [_p, _i, _psz],
     "lsph_generate_stream": [_p, _p, _i, _i, _i, _i, _p, _p, _p, C.c_float, _p, _p, _p, _p, _sz, _i, _p],
@@ -115,7 +113,6 @@ ARGTYPES = {
     # include/lspa.h (log-mel front end)
     "lspa_create": [_out_handle, _i],
     "lspa_load_mel_basis": [_p, _p, _i, _i],
-    "lspa_logmel": [_p, _p, _i64, _i, _i, C.c_double, _i, _p, _p],
     "lspa_logmel_at": [_p, _p, _i64, _i64, _i, _i, _i, C.c_double, _i, _p, _p],
     "lspa_destroy": [_p],
     "lspa_last_error": [],
@@ -133,7 +130,6 @@ ARGTYPES = {
     "lspr_create": [_out_handle, C.POINTER(LsprConfig), _i],
     "lspr_load_weights": [_p, _tensors, _i],
     "lspr_workspace_bytes": [_p, _i, _psz],
-    "lspr_forward": [_p, _p, _i, _p, _p, _sz, _i, _p],
     "lspr_state_bytes": [_p, _psz],
     "lspr_forward_stream": [_p, _p, _i, _i64, _p, _p, _p, _sz, _i, _p],
     "lspr_debug_packed": [_p, _i, _p, _pi64],
@@ -145,10 +141,6 @@ ARGTYPES = {
 def symbols(prefix: Optional[str] = None) -> List[str]:
     """The bound symbols of one module (``"lspm"``, ...), or of all six."""
     return [name for name in ARGTYPES if prefix is None or name.startswith(prefix + "_")]
-
-
-# Per-module names that callers outside the package (tests, scripts) use: views of the table and of check().
-SYMBOLS, SYMBOLS_H, SYMBOLS_M, SYMBOLS_A, SYMBOLS_L, SYMBOLS_R = (symbols(p) for p in ("lspg", "lsph", "lspm", "lspa", "lspl", "lspr"))
 
 
 class LspgError(RuntimeError):
@@ -197,9 +189,6 @@ def check(code: int, prefix: str = "lspg") -> None:
     """Raise ``LspgError`` with ``<prefix>_last_error()`` if a ``<prefix>_*`` call returned ``code != 0``."""
     if code != 0:
         raise LspgError(code, (getattr(load(), prefix + "_last_error")() or b"").decode("utf-8", "replace"))
-
-
-check_h, check_m, check_a, check_l, check_r = (functools.partial(check, prefix=p) for p in ("lsph", "lspm", "lspa", "lspl", "lspr"))
 
 
 def cuda_device(device, what: str) -> torch.device:

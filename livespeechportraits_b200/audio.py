@@ -122,8 +122,8 @@ class MelFrontEnd(_lib.Handle):
         n = 2 * int(a.shape[0] / 16000 * 60)
         out = torch.empty((n, self.n_mels), dtype=torch.float32, device=self.device)
         with self.cuda_stream() as stream:
-            self.call("logmel", a.data_ptr() if a.numel() else None, a.shape[0], n, frame_len, step, int(bool(normalize)),
-                      out.data_ptr() if n else None, stream)
+            self.call("logmel_at", a.data_ptr() if a.numel() else None, 0, a.shape[0], 0, n, frame_len, step,
+                      int(bool(normalize)), out.data_ptr() if n else None, stream)
         return out
 
 

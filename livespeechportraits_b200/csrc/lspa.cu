@@ -221,8 +221,8 @@ int lspa_load_mel_basis(lspa_handle h, const float* host_basis, int n_mels, int 
   return LSPG_OK;
 }
 
-static int logmel(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
-                  int n_windows, int frame_len, double step, int normalize, float* out, void* stream, const char* what) {
+int lspa_logmel_at(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
+                   int n_windows, int frame_len, double step, int normalize, float* out, void* stream) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
   if (n_samples < 0) return fail(LSPG_EINVAL, "n_samples must be >= 0 (got %lld)", static_cast<long long>(n_samples));
   if (n_windows < 0) return fail(LSPG_EINVAL, "n_windows must be >= 0 (got %d)", n_windows);
@@ -238,7 +238,7 @@ static int logmel(lspa_handle h, const float* audio, int64_t first_sample, int64
   if (n_windows > 0 && static_cast<int64_t>(static_cast<double>(first_window) * step) < first_sample)
     return fail(LSPG_EINVAL, "window %d starts at sample %lld, before the first sample given (%lld)", first_window,
                 static_cast<long long>(static_cast<double>(first_window) * step), static_cast<long long>(first_sample));
-  if (int rc = capi::require_device<Lspa>(h->device, what)) return rc;
+  if (int rc = capi::require_device<Lspa>(h->device, "lspa_logmel_at")) return rc;
   if (h->n_mels == 0) return fail(LSPG_ESTATE, "lspa_load_mel_basis has not been called");
   if (n_windows == 0) return LSPG_OK;
   DeviceGuard g(h->device);
@@ -248,17 +248,6 @@ static int logmel(lspa_handle h, const float* audio, int64_t first_sample, int64
       normalize ? 1 : 0, out);
   CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
-}
-
-int lspa_logmel(lspa_handle h, const float* audio, int64_t n_samples, int n_windows, int frame_len, double step,
-                int normalize, float* out, void* stream) {
-  return logmel(h, audio, 0, n_samples, 0, n_windows, frame_len, step, normalize, out, stream, "lspa_logmel");
-}
-
-int lspa_logmel_at(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
-                   int n_windows, int frame_len, double step, int normalize, float* out, void* stream) {
-  return logmel(h, audio, first_sample, n_samples, first_window, n_windows, frame_len, step, normalize, out, stream,
-                "lspa_logmel_at");
 }
 
 }  // extern "C"

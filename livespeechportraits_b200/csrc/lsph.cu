@@ -7,7 +7,7 @@
 // Here:
 //   * Nothing that depends only on the audio stays in the loop: audio_downsample of every audio row (two GEMMs, eval
 //     BatchNorm1d folded into the first one's epilogue) and the 2 x 14 conditioning 1x1 convolutions (one GEMM,
-//     [n_audio, 512] x [512, 14*256]) are computed once per clip.
+//     [n_audio, 512] x [512, 14*256]) are computed once per call, for every audio row it is given.
 //   * The WaveNet is evaluated INCREMENTALLY over absolute time t: per frame ONE new time step, each block reading its
 //     own input at t and at t - dilation from a per-layer history.  This is the same function as the reference's
 //     full-window forward: the receptive field of the last window position equals the window length (255), so the
@@ -347,9 +347,6 @@ struct lsph_ctx {
   float *d_w_start1 = nullptr, *d_b_start1 = nullptr, *d_w_start2 = nullptr, *d_b_start2 = nullptr;
   float *d_w_fg = nullptr, *d_w_rs = nullptr, *d_b_rs = nullptr;
   float *d_w_end1 = nullptr, *d_b_end1 = nullptr, *d_w_end2 = nullptr, *d_b_end2 = nullptr;
-  // scratch (grown on demand)
-  int cap_audio = 0;
-  float *d_ds1 = nullptr, *d_hist = nullptr;   // the hoisted path's workspace for cap_audio rows; the history ring
   std::vector<float*> owned;
   std::vector<float> packed[7];      // host copies of the packed arrays (lsph_debug_packed)
 };
@@ -411,8 +408,6 @@ int lsph_destroy(lsph_handle h) {
   if (h->device >= 0) {
     DeviceGuard g(h->device);
     for (float* p : h->owned) cudaFree(p);
-    for (float* p : {h->d_ds1, h->d_hist})
-      if (p) cudaFree(p);
   }
   delete h;
   return LSPG_OK;
@@ -533,78 +528,6 @@ static size_t hoisted_floats(const lsph_ctx* h, int n_audio, size_t off[3]) {
 
 static size_t state_floats(const lsph_ctx* h) { return static_cast<size_t>(h->L) * h->ring * kR + kMaxIn; }
 
-// Frames frame0 .. frame0 + n_frames - 1 (absolute steps from t0 = frame0 + rf - 1, or from 0 with the warm-up when
-// frame0 == 0) from audio rows arow0 .. arow0 + n_audio - 1.  h_state null: pre_headpose starts the loop and nothing is saved.
-static int run(lsph_handle h, const float* audio_feats, int arow0, int n_audio, int frame0, int n_frames,
-               const float* pre_headpose, const float* noise, const float* uniform, float sigma_scale, float* out_pred,
-               float* out_params, float* hist, float* h_state, float* ws, int cluster, cudaStream_t st) {
-  const lsph_config& c = h->cfg;
-  const int H = c.apc_hidden, L = h->L;
-  size_t off[3];
-  hoisted_floats(h, n_audio, off);
-  float *ds1 = ws + off[0], *ds2 = ws + off[1], *cond = ws + off[2];
-  // ---- hoisted audio path: downsample every row given, project it for every block
-  const dim3 blk(256);
-  const int mt = (n_audio + 63) / 64;
-  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, ds1, n_audio, H, 2 * H, 1, 0);
-  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, ds2, n_audio, H, H, 0, 0);
-  gemm_nt_kernel<><<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(ds2, h->d_w_cond, h->d_one, h->d_b_cond, cond, n_audio, L * 2 * kR, H, 0, 0);
-  CUDA_TRY(cudaGetLastError());
-  LoopParams p;
-  memset(&p, 0, sizeof(p));
-  p.w_start1 = h->d_w_start1; p.b_start1 = h->d_b_start1; p.w_start2 = h->d_w_start2; p.b_start2 = h->d_b_start2;
-  p.w_fg = h->d_w_fg; p.w_rs = h->d_w_rs; p.b_rs = h->d_b_rs;
-  p.w_end1 = h->d_w_end1; p.b_end1 = h->d_b_end1; p.w_end2 = h->d_w_end2; p.b_end2 = h->d_b_end2;
-  p.cond = cond; p.h_in = (h_state && frame0 > 0) ? h_state : nullptr; p.pre_headpose = pre_headpose;
-  p.noise = noise; p.uniform = uniform;
-  p.hist = hist; p.h_out = h_state; p.out_pred = out_pred; p.out_params = out_params;
-  p.L = L; p.in_ch = c.input_ch; p.O = h->O; p.ndim = c.ndim; p.ncenter = c.ncenter; p.gmm = c.loss_gmm;
-  p.n_audio = n_audio; p.arow0 = arow0; p.frame0 = frame0; p.rf = h->rf; p.ff = c.frame_future;
-  p.t0 = frame0 == 0 ? 0 : frame0 + h->rf - 1; p.t1 = frame0 + n_frames + h->rf - 1; p.ring = h->ring;
-  p.sigma_scale = sigma_scale;
-  for (int l = 0; l < L; ++l) p.dil[l] = h->dil[l];
-  if (cluster == 8) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(8); cfg.blockDim = dim3(16 * 32); cfg.dynamicSmemBytes = 0; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 8; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    CUDA_TRY(cudaLaunchKernelEx(&cfg, headpose_loop_kernel<8, 16>, p));
-  } else {
-    headpose_loop_kernel<1, 32><<<1, 32 * 32, 0, st>>>(p);
-    CUDA_TRY(cudaGetLastError());
-  }
-  return LSPG_OK;
-}
-
-int lsph_generate(lsph_handle h, const float* audio_feats, int n_audio, const float* pre_headpose, const float* noise,
-                  const float* uniform, float sigma_scale, float* out_pred, float* out_params, int cluster, void* stream) {
-  if (!h) return fail(LSPG_EINVAL, "null handle");
-  if (int rc = capi::require_device<Lsph>(h->device, "lsph_generate")) return rc;
-  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lsph_load_weights has not been called");
-  const lsph_config& c = h->cfg;
-  if (!audio_feats || !pre_headpose || !out_pred) return fail(LSPG_EINVAL, "null buffer");
-  if (c.loss_gmm && !noise) return fail(LSPG_EINVAL, "noise is required for the GMM loss (pass zeros for sigma_scale 0)");
-  const int nframe = n_audio - c.frame_future;
-  if (nframe < 1) return fail(LSPG_EINVAL, "need more than frame_future (%d) audio rows, got %d", c.frame_future, n_audio);
-  if (cluster == 0) cluster = 8;
-  if (cluster != 1 && cluster != 8) return fail(LSPG_EINVAL, "cluster must be 1 or 8 (got %d)", cluster);
-  DeviceGuard g(h->device);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (n_audio > h->cap_audio) {
-    CUDA_TRY(cudaDeviceSynchronize());
-    if (h->d_ds1) { cudaFree(h->d_ds1); h->d_ds1 = nullptr; }
-    const int cap = n_audio + 64;
-    size_t off[3];
-    CUDA_TRY(cudaMalloc(&h->d_ds1, sizeof(float) * hoisted_floats(h, cap, off)));
-    if (!h->d_hist) CUDA_TRY(cudaMalloc(&h->d_hist, sizeof(float) * state_floats(h)));
-    h->cap_audio = cap;
-  }
-  return run(h, audio_feats, 0, n_audio, 0, nframe, pre_headpose, noise, uniform, sigma_scale, out_pred, out_params, h->d_hist,
-             nullptr, h->d_ds1, cluster, st);
-}
-
 int lsph_state_bytes(lsph_handle h, size_t* bytes) {
   if (!h || !bytes) return fail(LSPG_EINVAL, "null argument");
   *bytes = sizeof(float) * state_floats(h);
@@ -649,10 +572,46 @@ int lsph_generate_stream(lsph_handle h, const float* audio_feats, int audio_row0
   if (!h->weights_loaded) return fail(LSPG_ESTATE, "lsph_load_weights has not been called");
   if (n_frames == 0) return LSPG_OK;
   DeviceGuard g(h->device);
-  float* hist = state;
-  float* h_state = state + static_cast<size_t>(h->L) * h->ring * kR;
-  return run(h, audio_feats, audio_row0, n_audio, frame0, n_frames, pre_headpose, noise, uniform, sigma_scale, out_pred,
-             out_params, hist, h_state, static_cast<float*>(ws), cluster, static_cast<cudaStream_t>(stream));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int H = c.apc_hidden, L = h->L;
+  float* w = static_cast<float*>(ws);
+  float *ds1 = w + off[0], *ds2 = w + off[1], *cond = w + off[2];
+  float* h_state = state + static_cast<size_t>(L) * h->ring * kR;     // after the history ring
+  // ---- hoisted audio path: downsample every row given, project it for every block
+  const dim3 blk(256);
+  const int mt = (n_audio + 63) / 64;
+  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(audio_feats, h->d_w_ds0, h->d_scale0, h->d_shift0, ds1, n_audio, H, 2 * H, 1);
+  gemm_nt_kernel<><<<dim3(H / 64, mt), blk, 0, st>>>(ds1, h->d_w_ds3, h->d_one, h->d_b_ds3, ds2, n_audio, H, H, 0);
+  gemm_nt_kernel<><<<dim3(L * 2 * kR / 64, mt), blk, 0, st>>>(ds2, h->d_w_cond, h->d_one, h->d_b_cond, cond, n_audio, L * 2 * kR, H, 0);
+  CUDA_TRY(cudaGetLastError());
+  // ---- the loop over frames frame0 .. frame0 + n_frames - 1: absolute steps from t0 = frame0 + rf - 1, or from 0 with
+  // the warm-up when frame0 == 0
+  LoopParams p;
+  memset(&p, 0, sizeof(p));
+  p.w_start1 = h->d_w_start1; p.b_start1 = h->d_b_start1; p.w_start2 = h->d_w_start2; p.b_start2 = h->d_b_start2;
+  p.w_fg = h->d_w_fg; p.w_rs = h->d_w_rs; p.b_rs = h->d_b_rs;
+  p.w_end1 = h->d_w_end1; p.b_end1 = h->d_b_end1; p.w_end2 = h->d_w_end2; p.b_end2 = h->d_b_end2;
+  p.cond = cond; p.h_in = frame0 > 0 ? h_state : nullptr; p.pre_headpose = pre_headpose;
+  p.noise = noise; p.uniform = uniform;
+  p.hist = state; p.h_out = h_state; p.out_pred = out_pred; p.out_params = out_params;
+  p.L = L; p.in_ch = c.input_ch; p.O = h->O; p.ndim = c.ndim; p.ncenter = c.ncenter; p.gmm = c.loss_gmm;
+  p.n_audio = n_audio; p.arow0 = audio_row0; p.frame0 = frame0; p.rf = h->rf; p.ff = c.frame_future;
+  p.t0 = frame0 == 0 ? 0 : frame0 + h->rf - 1; p.t1 = frame0 + n_frames + h->rf - 1; p.ring = h->ring;
+  p.sigma_scale = sigma_scale;
+  for (int l = 0; l < L; ++l) p.dil[l] = h->dil[l];
+  if (cluster == 8) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(8); cfg.blockDim = dim3(16 * 32); cfg.dynamicSmemBytes = 0; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 8; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr; cfg.numAttrs = 1;
+    CUDA_TRY(cudaLaunchKernelEx(&cfg, headpose_loop_kernel<8, 16>, p));
+  } else {
+    headpose_loop_kernel<1, 32><<<1, 32 * 32, 0, st>>>(p);
+    CUDA_TRY(cudaGetLastError());
+  }
+  return LSPG_OK;
 }
 
 }  // extern "C"

@@ -238,7 +238,7 @@ int max_clusters(K kernel, int cl, size_t smem, int* out) {
 
 void gemm(const float* A, const float* W, const float* scale, const float* shift, float* C, int M, int N, int K, int leaky,
           cudaStream_t st) {
-  gemm_nt_kernel<><<<dim3(N / 64, (M + 63) / 64), 256, 0, st>>>(A, W, scale, shift, C, M, N, K, leaky, 0);
+  gemm_nt_kernel<><<<dim3(N / 64, (M + 63) / 64), 256, 0, st>>>(A, W, scale, shift, C, M, N, K, leaky);
 }
 
 }  // namespace
@@ -394,7 +394,7 @@ int lspr_debug_packed(lspr_handle h, int which, float* dst, int64_t* count) {
 }
 
 // Workspace layout (floats, every block 64-float aligned).  APC: xproj [T][3H], two layer buffers [T][H].
-// MOUTH (Ls = n/2 + frame_future LSTM steps): two MLP buffers [Ls][max(D, 512)], xproj [Ls][4*256], two LSTM buffers [Ls][256].
+// MOUTH (T = n/2 LSTM steps): two MLP buffers [T][max(D, 512)], xproj [T][4*256], two LSTM buffers [T][256].
 static size_t workspace_floats(const lspr_ctx* h, int n_rows, size_t off[5]) {
   size_t T, sz[5];
   int nb;
@@ -402,7 +402,7 @@ static size_t workspace_floats(const lspr_ctx* h, int n_rows, size_t off[5]) {
     T = static_cast<size_t>(n_rows);
     sz[0] = T * h->G * h->H; sz[1] = sz[2] = T * h->H; nb = 3;
   } else {
-    T = static_cast<size_t>(n_rows / 2 + h->cfg.frame_future);
+    T = static_cast<size_t>(n_rows / 2);
     const size_t w = std::max(h->cfg.input_dim, kFcW);
     sz[0] = sz[1] = T * w; sz[2] = T * h->G * h->H; sz[3] = sz[4] = T * h->H; nb = 5;
   }
@@ -425,27 +425,19 @@ int lspr_state_bytes(lspr_handle h, size_t* bytes) {
   return LSPG_OK;
 }
 
-// The whole clip (state == nullptr: every layer starts from zeros, Audio2Mouth appends its frame_future pairs of the last
-// row) or one chunk of a stream (state: the layers' h and c, carried across calls; step0: global step of the chunk's first
-// row, APC, or pair, MOUTH).
-static int forward(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
-                   size_t ws_bytes, int cluster, void* stream, const char* what) {
+// One span of a clip: state holds the layers' h and c, carried across calls; step0 is the global step of the span's first
+// row (APC) or pair (MOUTH).  A whole clip is the span from step 0.
+int lspr_forward_stream(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
+                        size_t ws_bytes, int cluster, void* stream) {
   if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (!state) return fail(LSPG_EINVAL, "null state");
   const lspr_config& c = h->cfg;
   const bool apc = c.kind == LSPR_APC;
-  if (!state) {
-    if (int rc = capi::require_device<Lspr>(h->device, what)) return rc;
-    if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
-    if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
-    if (!apc && (n_rows < 2 || n_rows % 2))
-      return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even and >= 2 (got %d)", n_rows);
-  } else {
-    if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
-    if (!apc && n_rows % 2) return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even (got %d)", n_rows);
-    if (step0 < 0 || step0 > INT32_MAX) return fail(LSPG_EINVAL, "step0 must be in [0, 2^31) (got %lld)", static_cast<long long>(step0));
-  }
-  // a MOUTH chunk before frame_future returns no rows, so it may pass no output buffer
-  if (n_rows > 0 && (!in || (!out && (apc || !state || step0 + n_rows / 2 > c.frame_future))))
+  if (n_rows < 0) return fail(LSPG_EINVAL, "n_rows must be >= 0 (got %d)", n_rows);
+  if (!apc && n_rows % 2) return fail(LSPG_EINVAL, "Audio2Mouth reads APC rows in pairs: n_rows must be even (got %d)", n_rows);
+  if (step0 < 0 || step0 > INT32_MAX) return fail(LSPG_EINVAL, "step0 must be in [0, 2^31) (got %lld)", static_cast<long long>(step0));
+  // a MOUTH span before frame_future returns no rows, so it may pass no output buffer
+  if (n_rows > 0 && (!in || (!out && (apc || step0 + n_rows / 2 > c.frame_future))))
     return fail(LSPG_EINVAL, "null buffer");
   if ((reinterpret_cast<uintptr_t>(in) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(state)) % 16)
     return fail(LSPG_EINVAL, "in, out and state must be 16-byte aligned");
@@ -461,24 +453,21 @@ static int forward(lspr_handle h, const float* in, int n_rows, int64_t step0, fl
     if (cl == 0) cl = 8;
     if (cl != 8) return fail(LSPG_EINVAL, "Audio2Mouth cluster must be 0 or 8 (got %d)", cluster);
   }
-  if (state) {
-    if (int rc = capi::require_device<Lspr>(h->device, what)) return rc;
-    if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
-  }
+  if (int rc = capi::require_device<Lspr>(h->device, "lspr_forward_stream")) return rc;
+  if (!h->weights_loaded) return fail(LSPG_ESTATE, "lspr_load_weights has not been called");
   if ((cl == 16 ? h->max_clusters16 : h->max_clusters8) < 1)
     return fail(LSPG_ENODEV, "a %d-CTA cluster with %zu bytes of shared memory per CTA cannot be scheduled on device %d", cl,
                  cl == 16 ? kGru16Smem : (apc ? kGru8Smem : kLstm8Smem), h->device);
   DeviceGuard g(h->device);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int G = h->G, H = h->H;
-  if (state && step0 == 0) CUDA_TRY(cudaMemsetAsync(state, 0, sizeof(float) * static_cast<size_t>(h->L) * 2 * H, st));
+  if (step0 == 0) CUDA_TRY(cudaMemsetAsync(state, 0, sizeof(float) * static_cast<size_t>(h->L) * 2 * H, st));
   if (n_rows == 0) return LSPG_OK;
   float* w = static_cast<float*>(ws);
   auto P = [&](int i) { return static_cast<const float*>(h->d_packed[i]); };
   auto layer = [&](int l, const float* x, int T, float* xproj, float* dst, const float* resid) -> int {
     gemm(x, P(4 * l), h->d_ones, P(4 * l + 1), xproj, T, G * H, h->in_w[l], 0, st);
-    RecParams p{xproj, P(4 * l + 2), G == 3 ? P(4 * l + 3) : nullptr, resid, dst,
-                state ? state + static_cast<size_t>(l) * 2 * H : nullptr, T};
+    RecParams p{xproj, P(4 * l + 2), G == 3 ? P(4 * l + 3) : nullptr, resid, dst, state + static_cast<size_t>(l) * 2 * H, T};
     return launch_rnn(h, cl, p, st);
   };
   int r;
@@ -495,38 +484,27 @@ static int forward(lspr_handle h, const float* in, int n_rows, int64_t step0, fl
       x = dst;
     }
   } else {
-    // Whole clip: the LSTM runs nframe + frame_future steps, the last frame_future over copies of the last row, which the
-    // downsample GEMM reads by clamping.  A chunk runs one step per pair it is given (every pair whole: nothing clamps).
-    const int D = c.input_dim, ff = c.frame_future, np = n_rows / 2, Ls = state ? np : np + ff;
+    // One LSTM step per pair of rows: the downsample GEMM reads `in` as [n_rows / 2, 2 D] (models/audio2feature.py:65).
+    const int D = c.input_dim, ff = c.frame_future, np = n_rows / 2;
     // fc runs on the global steps >= frame_future (models/audio2feature_model.py:147 drops the first frame_future)
-    const int skip = state ? static_cast<int>(std::min<int64_t>(np, std::max<int64_t>(0, ff - step0))) : ff;
-    const int n_out = Ls - skip;
+    const int skip = static_cast<int>(std::min<int64_t>(np, std::max<int64_t>(0, ff - step0)));
+    const int n_out = np - skip;
     float *m0 = w + off[0], *m1 = w + off[1], *xproj = w + off[2], *la = w + off[3], *lb = w + off[4];
-    gemm_nt_kernel<false, true><<<dim3(D / 64, (Ls + 63) / 64), 256, 0, st>>>(in, P(12), P(13), P(14), m0, Ls, D, 2 * D, 1, n_rows);
-    gemm(m0, P(15), P(16), P(17), m1, Ls, D, D, 0, st);
-    if ((r = layer(0, m1, Ls, xproj, la, nullptr))) return r;
-    if ((r = layer(1, la, Ls, xproj, lb, nullptr))) return r;
-    if ((r = layer(2, lb, Ls, xproj, la, nullptr))) return r;
+    gemm(in, P(12), P(13), P(14), m0, np, D, 2 * D, 1, st);
+    gemm(m0, P(15), P(16), P(17), m1, np, D, D, 0, st);
+    if ((r = layer(0, m1, np, xproj, la, nullptr))) return r;
+    if ((r = layer(1, la, np, xproj, lb, nullptr))) return r;
+    if ((r = layer(2, lb, np, xproj, la, nullptr))) return r;
     if (n_out > 0) {
       const float* kept = la + static_cast<size_t>(skip) * kLstmH;
       gemm(kept, P(18), P(19), P(20), m0, n_out, kFcW, kLstmH, 1, st);
       gemm(m0, P(21), P(22), P(23), m1, n_out, kFcW, kFcW, 1, st);
-      gemm_nt_kernel<true, false><<<dim3((c.out_dim + 63) / 64, (n_out + 63) / 64), 256, 0, st>>>(m1, P(24), P(25), P(26), out,
-                                                                                                 n_out, c.out_dim, kFcW, 0, 0);
+      gemm_nt_kernel<true><<<dim3((c.out_dim + 63) / 64, (n_out + 63) / 64), 256, 0, st>>>(m1, P(24), P(25), P(26), out,
+                                                                                          n_out, c.out_dim, kFcW, 0);
     }
   }
   CUDA_TRY(cudaGetLastError());
   return LSPG_OK;
-}
-
-int lspr_forward(lspr_handle h, const float* in, int n_rows, float* out, void* ws, size_t ws_bytes, int cluster, void* stream) {
-  return forward(h, in, n_rows, 0, out, nullptr, ws, ws_bytes, cluster, stream, "lspr_forward");
-}
-
-int lspr_forward_stream(lspr_handle h, const float* in, int n_rows, int64_t step0, float* out, float* state, void* ws,
-                        size_t ws_bytes, int cluster, void* stream) {
-  if (h && !state) return fail(LSPG_EINVAL, "null state");
-  return forward(h, in, n_rows, step0, out, state, ws, ws_bytes, cluster, stream, "lspr_forward_stream");
 }
 
 }  // extern "C"

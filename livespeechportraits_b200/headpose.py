@@ -83,18 +83,39 @@ class HeadposeGenerator(_lib.Handle):
             raise ValueError(f"pre_headpose must have {self.cfg.input_ch} values")
         nz = to(noise).reshape(nframe, self.cfg.ndim) if noise is not None else torch.zeros((nframe, self.cfg.ndim), device=dev)
         un = to(uniform).reshape(nframe) if uniform is not None else None
-        pred = torch.empty((nframe, self.cfg.ndim), dtype=torch.float32, device=dev)
-        params = torch.empty((nframe, self.out_channels), dtype=torch.float32, device=dev) if return_params else None
         for t in (a, pre, nz):
             if t.data_ptr() % 16:
                 raise ValueError("device buffers must be 16-byte aligned")
-        with self.cuda_stream() as stream:
-            self.call("generate", a.data_ptr(), n_audio, pre.data_ptr(), nz.data_ptr(), un.data_ptr() if un is not None else None,
-                      float(sigma_scale), pred.data_ptr(), params.data_ptr() if params is not None else None, int(cluster),
-                      stream)
-        self._keep = (a, pre, nz, un)            # inputs stay alive until the caller synchronises on the result
+        pred, params, _ = self._run(a, 0, 0, nframe, pre, nz, un, float(sigma_scale), self._new_state(), None, return_params,
+                                    int(cluster))
         return (pred, params) if return_params else pred
 
+    def _new_state(self) -> torch.Tensor:
+        """A device buffer for the loop's state (include/lsph.h, ``lsph_state_bytes``); the call at frame 0 starts it."""
+        need = C.c_size_t()
+        self.call("state_bytes", C.byref(need))
+        return torch.empty(need.value // 4, dtype=torch.float32, device=self.device)
+
+    def _run(self, rows, row0: int, frame0: int, n: int, pre, noise, uniform, sigma_scale: float, state, ws,
+             return_params: bool, cluster: int):
+        """One ``lsph_generate_stream`` call: frames ``frame0 .. frame0 + n - 1`` from the device audio rows ``rows``
+        (global rows ``row0 ..``; fp32, contiguous, 16-byte aligned) with the draws ``noise`` [n, ndim] and ``uniform``
+        [n] (or None).  Returns pred [n, ndim], the network outputs [n, out_ch] (None without ``return_params``) and the
+        workspace used (``ws`` or a larger one; nothing runs for n == 0)."""
+        dev = self.device
+        pred = torch.empty((n, self.cfg.ndim), dtype=torch.float32, device=dev)
+        params = torch.empty((n, self.out_channels), dtype=torch.float32, device=dev) if return_params else None
+        if n:
+            need = C.c_size_t()
+            self.call("stream_workspace_bytes", rows.shape[0], C.byref(need))
+            ws = _lib.reserve(ws, need.value, dev)
+            ptr = lambda t: t.data_ptr() if t is not None else None    # noqa: E731
+            with self.cuda_stream() as stream:
+                self.call("generate_stream", rows.data_ptr(), row0, rows.shape[0], frame0, n, pre.data_ptr(), ptr(noise),
+                          ptr(uniform), sigma_scale, pred.data_ptr(), ptr(params), state.data_ptr(), ws.data_ptr(),
+                          ws.numel(), cluster, stream)
+            self._keep = (rows, pre, noise, uniform, state, ws)   # the buffers stay alive until the caller synchronises
+        return pred, params, ws
 
     def stream(self, pre_headpose=None, sigma_scale: float = 0.3, noise=None, return_params: bool = False,
                cluster: int = 0) -> "HeadposeStream":
@@ -125,9 +146,7 @@ class HeadposeStream:
         self._pre = _lib.to_device(pre, gen.device).reshape(-1)
         if self._pre.numel() != cfg.input_ch:
             raise ValueError(f"pre_headpose must have {cfg.input_ch} values")
-        need = C.c_size_t()
-        gen.call("state_bytes", C.byref(need))
-        self._state = torch.empty(need.value // 4, dtype=torch.float32, device=gen.device)
+        self._state = gen._new_state()
         self._ws = None                        # workspace of the hoisted GEMMs, kept across pushes
         self._rows = torch.empty((0, 2 * cfg.apc_hidden), dtype=torch.float32, device=gen.device)
         self._row0 = 0                         # global index of self._rows[0]
@@ -159,21 +178,10 @@ class HeadposeStream:
         if rows.data_ptr() % 16:
             rows = rows.clone()
         n = max(0, self.rows - cfg.frame_future) - self.frames
-        pred = torch.empty((n, cfg.ndim), dtype=torch.float32, device=dev)
-        params = torch.empty((n, self._gen.out_channels), dtype=torch.float32, device=dev) if self._params else None
-        if n:
-            noise, uniform = self._draws(n)
-            need = C.c_size_t()
-            self._gen.call("stream_workspace_bytes", rows.shape[0], C.byref(need))
-            ws = self._ws = _lib.reserve(self._ws, need.value, dev)
-            with self._gen.cuda_stream() as stream:
-                self._gen.call("generate_stream", rows.data_ptr(), self._row0, rows.shape[0], self.frames, n,
-                               self._pre.data_ptr(), noise.data_ptr() if noise is not None else None,
-                               uniform.data_ptr() if uniform is not None else None, self._sigma, pred.data_ptr(),
-                               params.data_ptr() if params is not None else None, self._state.data_ptr(), ws.data_ptr(),
-                               ws.numel(), self._cluster, stream)
-            self._keep = (rows, noise, uniform)
-            self.frames += n
+        noise, uniform = self._draws(n) if n else (None, None)
+        pred, params, self._ws = self._gen._run(rows, self._row0, self.frames, n, self._pre, noise, uniform, self._sigma,
+                                                self._state, self._ws, self._params, self._cluster)
+        self.frames += n
         keep = self.frames + cfg.frame_future if self.frames else 0          # the first row a later frame reads
         drop = min(max(keep - self._row0, 0), rows.shape[0])
         self._rows = rows[drop:].clone()

@@ -56,33 +56,24 @@ class _Recurrent(_lib.Handle):
         x = x.to(device=self.device, dtype=torch.float32).contiguous()
         return x.clone() if x.data_ptr() % 16 else x
 
-    def _run(self, x: torch.Tensor, width: int, out_shape, cluster: int) -> torch.Tensor:
-        x = self._input(x, width)
-        n = x.shape[0]
-        out = torch.empty(out_shape, dtype=torch.float32, device=self.device)
-        ws = self.workspace(n)
-        with self.cuda_stream() as stream:
-            self.call("forward", x.data_ptr(), n, out.data_ptr(), ws.data_ptr(), ws.numel(), int(cluster), stream)
-        self._keep = (x, ws)           # inputs stay alive until the caller synchronises on the result
-        return out
-
     def _new_state(self) -> torch.Tensor:
+        """Uninitialised: the call from step 0 zeroes it."""
         if self.device is None:
             raise RuntimeError("host-only handle: created with device=-1")
         need = C.c_size_t()
         self.call("state_bytes", C.byref(need))
-        return torch.zeros(need.value // 4, dtype=torch.float32, device=self.device)
+        return torch.empty(need.value // 4, dtype=torch.float32, device=self.device)
 
-    def _run_stream(self, x: torch.Tensor, step0: int, state: torch.Tensor, ws, n_out: int, out_dim: int, cluster: int):
-        """One ``lspr_forward_stream`` call: ``x`` [n, width] from global step ``step0``, with the stream's workspace
-        ``ws`` (grown if too small); returns ([n_out, out_dim], the workspace)."""
+    def _run(self, x: torch.Tensor, step0: int, state: torch.Tensor, ws, n_out: int, out_dim: int, cluster: int):
+        """One ``lspr_forward_stream`` call: ``x`` [n, width] from global step ``step0``, with the workspace ``ws``
+        (None, or grown if too small); returns ([n_out, out_dim], the workspace)."""
         n = x.shape[0]
         out = torch.empty((n_out, out_dim), dtype=torch.float32, device=self.device)
         ws = _lib.reserve(ws, self.workspace_bytes(n), self.device)
         with self.cuda_stream() as stream:
             self.call("forward_stream", x.data_ptr() if n else None, n, int(step0), out.data_ptr() if n_out else None,
                       state.data_ptr(), ws.data_ptr(), ws.numel(), int(cluster), stream)
-        self._keep = x
+        self._keep = (x, state, ws)    # the buffers stay alive until the caller synchronises on the result
         return out, ws
 
 
@@ -111,7 +102,8 @@ class ApcEncoder(_Recurrent):
     def forward(self, mel: torch.Tensor, cluster: int = 0) -> torch.Tensor:
         """mel [T, mel_dim] CUDA -> features [T, hidden] CUDA fp32, enqueued on the current stream.  ``cluster``: CTAs
         per recurrence launch (0 = library choice, 8 or 16)."""
-        return self._run(mel, self.mel_dim, (mel.shape[0], self.hidden), cluster)
+        x = self._input(mel, self.mel_dim)
+        return self._run(x, 0, self._new_state(), None, x.shape[0], self.hidden, cluster)[0]
 
     __call__ = forward
 
@@ -135,8 +127,7 @@ class ApcStream:
     def push(self, mel: torch.Tensor) -> torch.Tensor:
         """mel [n, mel_dim] CUDA (n >= 0) -> features [n, hidden] CUDA fp32."""
         x = self._enc._input(mel, self._enc.mel_dim)
-        out, self._ws = self._enc._run_stream(x, self.rows, self._state, self._ws, x.shape[0], self._enc.hidden,
-                                              self._cluster)
+        out, self._ws = self._enc._run(x, self.rows, self._state, self._ws, x.shape[0], self._enc.hidden, self._cluster)
         self.rows += x.shape[0]
         return out
 
@@ -177,7 +168,9 @@ class MouthGenerator(_Recurrent):
             raise RuntimeError(f"shape '[1, -1, {2 * self.apc_hidden}]' is invalid for input of size {total}")
         if n < 2:
             raise ValueError("need at least 2 APC rows")
-        return self._run(feats, self.apc_hidden, (n // 2, self.out_dim), 0)
+        x = self._input(feats, self.apc_hidden)
+        x = torch.cat([x, x[-1:].expand(2 * self.frame_future, -1)])    # models/audio2feature_model.py:134
+        return self._run(x, 0, self._new_state(), None, n // 2, self.out_dim, 0)[0]
 
     def stream(self) -> "MouthStream":
         """A stream over one clip's APC features: ``push(feats)`` returns the track rows whose inputs are all in (frame f
@@ -204,7 +197,7 @@ class MouthStream:
     def _run(self, x: torch.Tensor) -> torch.Tensor:
         ff, np_ = self._gen.frame_future, x.shape[0] // 2
         n_out = max(0, self.pairs + np_ - max(self.pairs, ff))          # the new global steps >= frame_future
-        out, self._ws = self._gen._run_stream(x, self.pairs, self._state, self._ws, n_out, self._gen.out_dim, 0)
+        out, self._ws = self._gen._run(x, self.pairs, self._state, self._ws, n_out, self._gen.out_dim, 0)
         self.pairs += np_
         self.frames += n_out
         return out

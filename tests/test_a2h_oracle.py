@@ -159,8 +159,11 @@ def test_c_abi_exports_and_argument_checks():
     if not torch.cuda.is_available():
         assert lib.lsph_create(C.byref(h), C.byref(cfg), 0) == -2                      # no device, no fallback
     assert lib.lsph_create(C.byref(h), C.byref(cfg), -1) == 0
-    buf = (C.c_float * 4)()
-    assert lib.lsph_generate(h, buf, 40, buf, buf, None, 0.3, buf, None, 0, None) == -2 and b"no CPU path" in lib.lsph_last_error()
+    buf, P = (C.c_float * 4)(), 1 << 12                                               # P: a 256-byte aligned stand-in (never read)
+    ws = C.c_size_t()
+    assert lib.lsph_stream_workspace_bytes(h, 40, C.byref(ws)) == 0
+    assert lib.lsph_generate_stream(h, buf, 0, 40, 0, 25, buf, buf, None, 0.3, buf, None, P, P, ws.value, 0, None) == -2 \
+        and b"no CPU path" in lib.lsph_last_error()
     arr = (_lib.LspgTensor * 1)()
     w = torch.zeros(512, 1024)
     arr[0].name, arr[0].data, arr[0].numel = b"audio_downsample.0.weight", C.cast(w.data_ptr(), C.POINTER(C.c_float)), w.numel()

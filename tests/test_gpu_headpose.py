@@ -72,6 +72,28 @@ def test_full_clip_cluster_vs_single_cta_and_oracle_sample():
     assert np.array_equal(again, p8)                        # deterministic
 
 
+def test_two_cuda_streams_share_one_generator():
+    """Two different clips through one generator, enqueued on two CUDA streams with no synchronisation between the
+    enqueues: every call owns its loop state and workspace, so each output equals its serial result bit for bit."""
+    opt = A.default_opt()
+    g = _gen(opt, A.make_state_dict(opt, "B", 1))
+    dev = g.device
+    clips = [(torch.from_numpy(A.make_audio_feats(n, opt, seed)).to(dev),
+              torch.from_numpy(A.reference_noise(n - opt.frame_future, 12, 1, seed=seed)).to(dev))
+             for n, seed in ((687, 2), (400, 5))]
+    pre = torch.zeros(12, device=dev)
+    serial = [g.generate(a, pre, nz, 0.3) for a, nz in clips]
+    torch.cuda.synchronize()
+    streams = [torch.cuda.Stream(dev) for _ in clips]
+    concurrent = []
+    for s, (a, nz) in zip(streams, clips):
+        s.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(s):
+            concurrent.append(g.generate(a, pre, nz, 0.3))
+    torch.cuda.synchronize()
+    assert all(torch.equal(c, r) for c, r in zip(concurrent, serial))
+
+
 def test_drop_in_generate_sequences_keeps_signature_and_random_stream():
     import types
     from livespeechportraits_b200 import headpose

@@ -157,7 +157,7 @@ def test_host_only_handle_argument_checks():
         assert load(1, 257) == -2 and load(128, 257) == -2
         buf = (C.c_float * 16)()
         p = C.cast(buf, C.c_void_p)
-        mel = lambda a, n, nw, L, step=133.33333333333334, out=p: lib.lspa_logmel(h, a, n, nw, L, step, 1, out, None)   # noqa: E731
+        mel = lambda a, n, nw, L, step=133.33333333333334, out=p: lib.lspa_logmel_at(h, a, 0, n, 0, nw, L, step, 1, out, None)   # noqa: E731
         for L in (189, 267, 0, -5, 512):
             assert mel(p, 20000, 10, L) == -1, L
         assert b"frame_len" in lib.lspa_last_error()

@@ -114,10 +114,11 @@ def test_host_only_handle_and_config_checks():
     enc = ApcEncoder(sd, device=-1)
     with pytest.raises(RuntimeError, match="CUDA tensor"):
         enc.forward(torch.zeros(4, 80))
-    assert lib.lspr_forward(enc._handle, None, 0, None, None, 0, 0, None) == -2          # LSPG_ENODEV: host-only handle
+    state = 1 << 12                                                                      # a stand-in pointer (never read)
+    assert lib.lspr_forward_stream(enc._handle, None, 0, 0, None, state, None, 0, 0, None) == -2   # LSPG_ENODEV: host-only handle
     assert "host-only" in (lib.lspr_last_error() or b"").decode()
     n = C.c_size_t()
-    _lib.check_r(lib.lspr_workspace_bytes(enc._handle, 100, C.byref(n)))
+    _lib.check(lib.lspr_workspace_bytes(enc._handle, 100, C.byref(n)), "lspr")
     assert n.value == 4 * (100 * 1536 + 2 * 51200)
     bad = dict(sd)
     del bad["rnns.2.bias_hh_l0"]

@@ -342,6 +342,11 @@ def test_stream_symbols_are_bound():
                  "lsph_stream_workspace_bytes", "lsph_generate_stream"):
         assert name in _lib.ARGTYPES
         assert getattr(_lib.load(), name).argtypes == _lib.ARGTYPES[name]
+    # a whole clip is the span from 0: the library exports no second entry point for it, so a caller of the old
+    # whole-clip signatures fails at symbol lookup instead of passing the wrong arguments
+    for name in ("lspa_logmel", "lspr_forward", "lsph_generate"):
+        assert name not in _lib.ARGTYPES
+        assert not hasattr(_lib.load(), name)
 
 
 def test_stream_calls_on_host_only_handles():
