@@ -46,6 +46,34 @@ int lspa_load_mel_basis(lspa_handle h, const float* host_basis, int n_mels, int 
 int lspa_logmel_at(lspa_handle h, const float* audio, int64_t first_sample, int64_t n_samples, int first_window,
                    int n_windows, int frame_len, double step, int normalize, float* out, void* stream);
 
+/* The resampling step of librosa.load (resampy.resample with a kaiser table, then resample_f), from native-rate frames
+ * to the rate sample_ratio * orig_sr.
+ *
+ * lspa_load_resample_filter: the filter for one sample_ratio = float(sr_new) / sr_orig, as resampy hands it to
+ * resample_f: host fp64 win[nwin] (the half window, already multiplied by sample_ratio when sample_ratio < 1), delta[nwin]
+ * (win[j + 1] - win[j], delta[nwin - 1] = 0) and num_table (table entries per zero crossing, 2^precision).  Synchronous:
+ * copies to a library-owned device buffer; a second call replaces the filter. */
+int lspa_load_resample_filter(lspa_handle h, const double* win, const double* delta, int nwin, int num_table,
+                              double sample_ratio);
+
+#define LSPA_FMT_F32 0 /* float32 samples */
+#define LSPA_FMT_S16 1 /* PCM16 samples, decoded as s / 32768 */
+
+/* Outputs first_out .. first_out + n_out - 1 of a clip into out (device fp32 [n_out]), with the loaded filter.
+ * frames: device [n_in, channels] interleaved (format LSPA_FMT_F32 or LSPA_FMT_S16, channels 1 or 2) holding the clip's
+ * frames [first_in, first_in + n_in); each frame is decoded and mixed to mono as librosa.load does (fp32 (c0 + c1) / 2).
+ * Frames outside the buffer read as zero: before frame 0 and after the clip's end that is what the reference's wing
+ * clamps compute, so the arithmetic does not depend on the clip's length, only the output count does
+ * (int(n * sample_ratio)).  reg_table: host int64 [n_reg][4], the time register of output t in closed form per binade:
+ * row {t_b, base, k, e} gives register(t) = (base + (t - t_b) * k) * 2^e for t_b <= t < the next row's t_b; row 0 starts
+ * at t_b = 0 and the last row {t_end, 0, 0, 0} ends the table, which must reach first_out + n_out.  Output t is
+ * resample_f's sum over the left wing, then the right wing, each tap an fp64 product and sum rounded to fp32.
+ * LSPG_EINVAL for bad counts, formats or channels, a malformed table, or first_in > 0 when output first_out's left wing
+ * can read before first_in (n - (nwin / index_step - 1) < first_in, n = (int64_t)register(first_out)).  Asynchronous on
+ * `stream`; allocates nothing. */
+int lspa_resample_at(lspa_handle h, const void* frames, int format, int channels, int64_t first_in, int64_t n_in,
+                     int64_t first_out, int64_t n_out, const int64_t* reg_table, int n_reg, float* out, void* stream);
+
 int lspa_destroy(lspa_handle h);
 const char* lspa_last_error(void);
 

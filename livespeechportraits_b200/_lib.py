@@ -114,6 +114,8 @@ ARGTYPES = {
     "lspa_create": [_out_handle, _i],
     "lspa_load_mel_basis": [_p, _p, _i, _i],
     "lspa_logmel_at": [_p, _p, _i64, _i64, _i, _i, _i, C.c_double, _i, _p, _p],
+    "lspa_load_resample_filter": [_p, _p, _p, _i, _i, C.c_double],
+    "lspa_resample_at": [_p, _p, _i, _i, _i64, _i64, _i64, _i64, _p, _i, _p, _p],
     "lspa_destroy": [_p],
     "lspa_last_error": [],
     # include/lspl.h (landmark post-processing, demo.py stage 5)

@@ -10,10 +10,15 @@ numpy restatement of it otherwise.
 
 ``install()`` patches ``compute_mel_one_sequence`` of the reference's ``funcs.utils`` module; ``demo.py`` calls it as a
 module attribute, so it then runs unchanged.  There is no CPU path.
+
+The step in front of it, ``librosa.load(path, sr=16000)`` (demo.py:179), is ``Resampler`` / ``load_wav``: the mono mix and
+resampy's ``kaiser_best`` resampling of native-rate audio, whole clips and live (``Resampler.stream``), in one kernel.
 """
 from __future__ import annotations
 
-from typing import Optional
+import functools
+import math
+from typing import Optional, Tuple
 
 import numpy as np
 import torch
@@ -186,6 +191,252 @@ class MelStream:
         self._tail0 = keep
         self._keep = buf
         return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Resampling to 16 kHz: librosa.load's to_mono + resampy.resample (kaiser tables) + fix_length
+# ------------------------------------------------------------------------------------------------------------------
+SR = 16000
+# resampy's shipped tables: num_zeros, precision (2^precision entries per zero crossing), Kaiser beta, rolloff
+RESAMPLE_FILTERS = {"kaiser_best": (64, 9, 14.769656459379492, 0.9475937167399596),
+                    "kaiser_fast": (16, 9, 8.555504641634386, 0.85)}
+REGISTER_HORIZON = 1 << 40      # outputs the register table covers: about 2.2 years at 16 kHz
+
+
+def resample_filter(name: str = "kaiser_best") -> Tuple[np.ndarray, int]:
+    """resampy's half window (fp64 [num_zeros * num_table + 1]) and num_table for the filter ``name``: resampy's own
+    table when resampy imports, else its ``sinc_window`` restated with ``scipy.signal.windows.kaiser``
+    (``taper[n:] * rolloff * sinc(rolloff * linspace(0, num_zeros, n + 1))``, n = num_table * num_zeros), which may
+    differ from the shipped ``.npz`` in the last bits.  The table is an input of ``Resampler``, like ``mel_basis``."""
+    if name not in RESAMPLE_FILTERS:
+        raise ValueError(f"unknown filter {name!r}; supported: {sorted(RESAMPLE_FILTERS)}")
+    try:
+        from resampy.filters import get_filter
+    except ImportError:
+        return _sinc_window(*RESAMPLE_FILTERS[name])
+    win, num_table, _ = get_filter(name)
+    return np.asarray(win, np.float64), int(num_table)
+
+
+@functools.lru_cache(maxsize=None)
+def _sinc_window(num_zeros, precision, beta, rolloff):
+    from scipy.signal.windows import kaiser
+    num_table = 2 ** precision
+    n = num_table * num_zeros
+    sinc_win = rolloff * np.sinc(rolloff * np.linspace(0, num_zeros, num=n + 1, endpoint=True))
+    taper = kaiser(2 * n + 1, beta)[n:]
+    win = taper * sinc_win
+    win.flags.writeable = False
+    return win, num_table
+
+
+def filter_shape(orig_sr: int, res_type: str = "kaiser_best", sr: int = SR) -> Tuple[int, int, int]:
+    """(nwin, num_table, index_step) of ``res_type`` at ``orig_sr -> sr``, from the table's parameters alone."""
+    num_zeros, precision = RESAMPLE_FILTERS[res_type][:2]
+    num_table = 2 ** precision
+    return num_zeros * num_table + 1, num_table, int(min(1.0, float(sr) / orig_sr) * num_table)
+
+
+@functools.lru_cache(maxsize=16)
+def register_table(sample_ratio: float, n_out: int = REGISTER_HORIZON) -> np.ndarray:
+    """resample_f's time register (``time_register += 1 / sample_ratio``, an fp64 running sum from 0.0) for outputs
+    0 .. n_out - 1, in closed form per binade: int64 rows ``(t_b, base, k, e)`` with register(t) = (base + (t - t_b) k)
+    2^e for t_b <= t < the next row's t_b, and a last row ``(n_out, 0, 0, 0)``.
+
+    Within the binade [2^(e+52), 2^(e+53)) every sum is a multiple of the ulp 2^e and each step adds the increment
+    rounded to that grid: a constant number of ulps, except that a tie may round the first step to the other parity
+    (after it the register is even and stays so).  So the row starts where the next two steps agree and runs to the
+    binade's end; a step that does not (the first, a parity fix, a step into the next binade) gets a one-output row and
+    is taken by a real fp64 add.  A few rows per binade: O(log n_out) in all."""
+    inc = 1.0 / sample_ratio
+    rows, t, reg = [], 0, 0.0
+    while t < n_out:
+        if reg == 0.0:
+            rows.append((t, 0, 0, 0))
+            t, reg = t + 1, reg + inc
+            continue
+        e = math.frexp(reg)[1] - 53                    # reg in [2^(e+52), 2^(e+53)), ulp 2^e
+        base = int(math.ldexp(reg, -e))
+        r1 = reg + inc
+        r2 = r1 + inc
+        if r2 < math.ldexp(1.0, e + 53) and r2 - r1 == r1 - reg:
+            k = int(math.ldexp(r1 - reg, -e))
+            steps = min(-(-((1 << 53) - base) // k), n_out - t)          # outputs t .. t + steps - 1 in this binade
+            rows.append((t, base, k, e))
+            t, reg = t + steps, math.ldexp(float(base + (steps - 1) * k), e) + inc
+        else:
+            rows.append((t, base, 0, e))
+            t, reg = t + 1, r1
+    rows.append((n_out, 0, 0, 0))
+    out = np.array(rows, dtype=np.int64)
+    out.flags.writeable = False
+    return out
+
+
+def register_at(table: np.ndarray, t) -> np.ndarray:
+    """The registers of outputs ``t`` (int array) from ``register_table`` rows, as the kernel evaluates them."""
+    t = np.asarray(t, np.int64)
+    r = np.searchsorted(table[:-1, 0], t, side="right") - 1
+    return np.ldexp((table[r, 1] + (t - table[r, 0]) * table[r, 2]).astype(np.float64), table[r, 3].astype(np.int32))
+
+
+def _frames(samples, channels: int) -> torch.Tensor:
+    """``samples`` (numpy or torch; [n] or [n, channels]; fp32 or int16) as a tensor, refused with ``ValueError``
+    otherwise.  Left on its device."""
+    a = torch.as_tensor(samples)
+    if a.dtype not in (torch.float32, torch.int16):
+        raise ValueError(f"samples must be float32 or int16 (got {a.dtype})")
+    if not (a.dim() == 1 and channels == 1) and not (a.dim() == 2 and a.shape[1] == channels):
+        raise ValueError(f"samples must be [n] (mono) or [n, channels] with channels = {channels}, got shape {tuple(a.shape)}")
+    return a
+
+
+class Resampler(_lib.Handle):
+    """``librosa.load``'s mono mix and resampling for audio decoded at ``orig_sr`` with ``channels`` (1 or 2) channels:
+    ``resample(samples)`` returns what ``librosa.load(path, sr=16000)`` returns for those samples, as a CUDA fp32
+    tensor.  The filter is resampy's ``res_type`` table (``resample_filter``), multiplied by the ratio when it is below
+    one; its device copy is taken at construction.  Sample formats: float32 and PCM16 (decoded as s / 32768, as
+    soundfile does), interleaved.  At ``orig_sr == 16000`` the mono mix is returned unchanged, as librosa does."""
+    prefix, what = "lspa", "the resampler"
+
+    def __init__(self, orig_sr: int, channels: int = 1, res_type: str = "kaiser_best", sr: int = SR,
+                 device: Optional[torch.device] = None):
+        if int(orig_sr) != orig_sr or orig_sr <= 0 or int(sr) != sr or sr <= 0:
+            raise ValueError(f"sample rates must be positive integers (got {orig_sr}, {sr})")
+        if channels not in (1, 2):
+            raise ValueError(f"channels must be 1 or 2 (got {channels})")
+        super().__init__(device)
+        self.orig_sr, self.sr, self.channels, self.res_type = int(orig_sr), int(sr), int(channels), res_type
+        self.sample_ratio = float(sr) / orig_sr
+        self._create()
+        if self.orig_sr == self.sr:
+            return
+        win, num_table = resample_filter(res_type)
+        win = np.array(win, np.float64)
+        if self.sample_ratio < 1:
+            win *= self.sample_ratio
+        delta = np.zeros_like(win)
+        delta[:-1] = np.diff(win)
+        self.nwin, self.num_table = win.shape[0], num_table
+        self.index_step = int(min(1.0, self.sample_ratio) * num_table)
+        self.wing = self.nwin // self.index_step     # the most taps of one wing
+        self.call("load_resample_filter", win.ctypes.data, delta.ctypes.data, self.nwin, num_table, self.sample_ratio)
+        self._reg = register_table(self.sample_ratio)
+
+    def n_out(self, n_in: int) -> int:
+        """``int(n_in * sample_ratio)``: the outputs resampy computes from ``n_in`` frames (it refuses fewer than one)."""
+        return int(n_in * self.sample_ratio)
+
+    def resample(self, samples) -> torch.Tensor:
+        """CUDA fp32 ``[ceil(n * sample_ratio)]`` for ``n`` frames ([n] or [n, channels], numpy or torch, fp32 or int16).
+        ``ValueError`` where resampy raises (fewer than one output).  Enqueued on the current stream; a host array goes
+        through pinned memory, so there is no host synchronisation."""
+        a = _frames(samples, self.channels)
+        n = a.shape[0]
+        if self.orig_sr == self.sr:
+            return mono_mix(_lib.to_device(a, self.device, a.dtype))
+        m = self.n_out(n)
+        if m < 1:
+            raise ValueError(f"input signal length={n} is too small to resample from {self.orig_sr}->{self.sr}")
+        a = _lib.to_device(a, self.device, a.dtype)
+        out = torch.empty(int(math.ceil(n * self.sample_ratio)), dtype=torch.float32, device=self.device)
+        out[m:] = 0.0
+        self._span(a, 0, 0, m, out)
+        return out
+
+    def _span(self, frames: torch.Tensor, first_in: int, first_out: int, n_out: int, out: torch.Tensor) -> None:
+        fmt = 1 if frames.dtype == torch.int16 else 0
+        with self.cuda_stream() as stream:
+            self.call("resample_at", frames.data_ptr() if frames.numel() else None, fmt, self.channels, first_in,
+                      frames.shape[0], first_out, n_out, self._reg.ctypes.data, self._reg.shape[0],
+                      out.data_ptr() if n_out else None, stream)
+
+    def stream(self) -> "ResampleStream":
+        """A stream over one clip's native-rate frames: ``push(frames)`` returns the 16 kHz samples that became final,
+        ``finish()`` the rest.  The concatenation equals ``resample`` of all the frames, bit for bit."""
+        return ResampleStream(self)
+
+
+def mono_mix(frames: torch.Tensor) -> torch.Tensor:
+    """librosa's decoding and ``to_mono`` on device frames: fp32 s / 32768 for PCM16, then fp32 (c0 + c1) / 2."""
+    x = frames.to(torch.float32) / 32768.0 if frames.dtype == torch.int16 else frames
+    return x if x.dim() == 1 else (x[:, 0] + x[:, 1]) / 2.0
+
+
+class ResampleStream:
+    """``Resampler.resample`` over frames pushed in pieces.  Output t is returned by the push after which every input
+    frame its right wing can read is in (``stream.resample_counts``): about ``nwin / index_step`` frames of latency,
+    4 ms at 48 kHz with ``kaiser_best``.  ``finish()`` returns the outputs that read past the clip's end and the
+    ``fix_length`` zero.  Only the frames from the left wing of the next output on are kept on the device."""
+
+    def __init__(self, rs: Resampler):
+        self._rs = rs
+        self.frames = 0                         # frames pushed so far
+        self.samples = 0                        # outputs returned so far
+        self.finished = False
+        self._tail = None                       # frames tail0 .. frames - 1
+        self._tail0 = 0
+
+    def push(self, frames) -> torch.Tensor:
+        """[m] or [m, channels] frames (numpy or torch, fp32 or int16, one format per stream) -> the new 16 kHz samples."""
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        a = _frames(frames, self._rs.channels)
+        if self._tail is not None and a.dtype != self._tail.dtype:
+            raise ValueError(f"one sample format per stream ({self._tail.dtype} so far, got {a.dtype})")
+        a = _lib.to_device(a, self._rs.device, a.dtype)
+        self.frames += a.shape[0]
+        buf = torch.cat([self._tail, a]) if self._tail is not None and self._tail.numel() else a
+        return self._emit(buf, False)
+
+    def finish(self) -> torch.Tensor:
+        """The rest, including ``fix_length``'s zero; ``ValueError`` where resampy would refuse the whole clip."""
+        if self.finished:
+            raise RuntimeError("the stream has finished")
+        self.finished = True
+        if self._rs.orig_sr != self._rs.sr and self._rs.n_out(self.frames) < 1:
+            raise ValueError(f"input signal length={self.frames} is too small to resample from {self._rs.orig_sr}->"
+                             f"{self._rs.sr}")
+        buf = self._tail if self._tail is not None else torch.empty(0, dtype=torch.float32, device=self._rs.device)
+        return self._emit(buf, True)
+
+    def _emit(self, buf: torch.Tensor, finished: bool) -> torch.Tensor:
+        from .stream import resample_counts
+        rs = self._rs
+        if rs.orig_sr == rs.sr:
+            self.samples = self.frames
+            self._tail = buf[:0]
+            return mono_mix(buf)
+        ready = resample_counts(self.frames, finished, rs.orig_sr, rs.res_type, rs.sr)
+        computed = min(ready, rs.n_out(self.frames))          # beyond it: fix_length's zero
+        out = torch.empty(ready - self.samples, dtype=torch.float32, device=rs.device)
+        out[computed - self.samples:] = 0.0
+        if computed > self.samples:
+            rs._span(buf, self._tail0, self.samples, computed - self.samples, out)
+        self.samples = ready
+        if finished:
+            self._tail = buf[:0]
+            return out
+        keep = int(register_at(rs._reg, ready)) - (rs.wing - 1)     # the left wing of the next output starts here
+        keep = min(max(keep, self._tail0), self.frames)
+        self._tail = buf[keep - self._tail0:].clone()
+        self._tail0 = keep
+        return out
+
+
+def load_wav(path: str, sr: int = SR, res_type: str = "kaiser_best", device: Optional[torch.device] = None) -> torch.Tensor:
+    """``librosa.load(path, sr=sr)`` for PCM16 and float32 WAV files with one or two channels, read with
+    ``scipy.io.wavfile``: CUDA fp32 ``[ceil(n * sr / orig_sr)]``.  Other sample formats and more channels are refused
+    with ``ValueError``."""
+    from scipy.io import wavfile
+    orig_sr, data = wavfile.read(path)
+    if data.dtype not in (np.int16, np.float32):
+        raise ValueError(f"{path}: {data.dtype} samples; only PCM16 and float32 WAV files are supported")
+    if data.ndim > 2 or (data.ndim == 2 and data.shape[1] > 2):
+        raise ValueError(f"{path}: {data.shape[1]} channels; at most two are supported")
+    if data.ndim == 2 and data.shape[1] == 1:
+        data = data[:, 0]
+    return Resampler(orig_sr, 1 if data.ndim == 1 else 2, res_type, sr, device).resample(np.ascontiguousarray(data))
 
 
 def compute_mel_one_sequence(audio, hop_length=int(16000 / 120), winlen=1 / 60, winstep=0.5 / 60, sr=16000, fps=60,

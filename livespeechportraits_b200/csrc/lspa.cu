@@ -21,6 +21,7 @@
 // No atomics and a fixed summation order everywhere: results are bit-identical from run to run.
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cmath>
 
 #include "../../include/lspa.h"
@@ -153,6 +154,83 @@ __global__ void __launch_bounds__(kThreads) lspa_logmel_kernel(const float* __re
   for (int e = tid; e < nw * n_mels; e += kThreads) dst[e] = stage[e];
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// librosa.load's resampling (resampy.resample_f with a kaiser table): one thread per output sample.
+//
+// The time register of output t is the reference's running fp64 sum 0 + 1/r + 1/r + ..., evaluated from a host table
+// of its closed form per binade: rows t_b, base, k, e with register(t) = (base + (t - t_b) k) 2^e for t_b <= t < the
+// next row's t_b.  The int64 product is exact (< 2^53) and the scaling by 2^e is exact, so the value is the serial
+// sum's bits.  Each tap is the reference's fp64 expression, weight = win[j] + eta delta[j], y = fp32(y + weight x), with
+// explicit _rn intrinsics so that nvcc contracts nothing into a DFMA.  Inputs before sample 0 or outside the buffer read
+// as +0, which leaves y unchanged: the same bits as the reference's wing clamps.
+constexpr int kRsThreads = 256;
+constexpr int kMaxRegRows = 64;                // register rows per launch; a span over more rows is split
+
+struct RegRows {
+  int n;
+  int64_t t0[kMaxRegRows], base[kMaxRegRows], k[kMaxRegRows];
+  int e[kMaxRegRows];
+};
+
+__device__ __forceinline__ double pow2(int e) { return __longlong_as_double(static_cast<long long>(e + 1023) << 52); }
+
+// Frame j of the buffer (clip frame first_in + j) decoded as soundfile does and mixed to mono as librosa's to_mono.
+template <int FMT, int CH>
+__device__ __forceinline__ float mono_at(const void* frames, int64_t j) {
+  float c[CH];
+#pragma unroll
+  for (int q = 0; q < CH; ++q) {
+    if (FMT == LSPA_FMT_S16)
+      c[q] = __fmul_rn(static_cast<float>(__ldg(static_cast<const short*>(frames) + j * CH + q)), 1.0f / 32768.0f);
+    else
+      c[q] = __ldg(static_cast<const float*>(frames) + j * CH + q);
+  }
+  return CH == 1 ? c[0] : __fmul_rn(__fadd_rn(c[0], c[CH - 1]), 0.5f);
+}
+
+// One wing: n_taps taps from table entry `offset` in steps of index_step, input frames p0, p0 + dir, ...
+template <int FMT, int CH>
+__device__ __forceinline__ float wing(float y, const double2* __restrict__ tab, int offset, int index_step, int n_taps,
+                                      double eta, const void* frames, int64_t p0, int dir, int64_t n_in) {
+#pragma unroll 4
+  for (int i = 0; i < n_taps; ++i) {
+    const double2 wd = __ldg(tab + offset + i * index_step);                 // (win, delta)
+    const double weight = __dadd_rn(wd.x, __dmul_rn(eta, wd.y));
+    const int64_t p = p0 + static_cast<int64_t>(dir) * i;
+    const float x = (p >= 0 && p < n_in) ? mono_at<FMT, CH>(frames, p) : 0.0f;
+    y = __double2float_rn(__dadd_rn(static_cast<double>(y), __dmul_rn(weight, static_cast<double>(x))));
+  }
+  return y;
+}
+
+// Outputs first_out .. first_out + n_out - 1 into out[0 ..]; frames holds clip frames [first_in, first_in + n_in).
+template <int FMT, int CH>
+__global__ void __launch_bounds__(kRsThreads) lspa_resample_kernel(const void* __restrict__ frames, int64_t first_in,
+                                                                   int64_t n_in, int64_t first_out, int64_t n_out,
+                                                                   RegRows reg, const double2* __restrict__ tab,
+                                                                   int nwin, int num_table, int index_step, double scale,
+                                                                   float* __restrict__ out) {
+  const int64_t o = static_cast<int64_t>(blockIdx.x) * kRsThreads + threadIdx.x;
+  if (o >= n_out) return;
+  const int64_t t = first_out + o;
+  int r = 0;                                   // the last row with t0 <= t
+  for (int s = kMaxRegRows / 2; s; s >>= 1)
+    if (r + s < reg.n && reg.t0[r + s] <= t) r += s;
+  const double tr = __dmul_rn(static_cast<double>(reg.base[r] + (t - reg.t0[r]) * reg.k[r]), pow2(reg.e[r]));
+  const int64_t n = static_cast<int64_t>(tr);
+  const double dn = static_cast<double>(n);
+  const double frac = __dmul_rn(scale, __dsub_rn(tr, dn));
+  double index_frac = __dmul_rn(frac, static_cast<double>(num_table));
+  int offset = static_cast<int>(index_frac);
+  double eta = __dsub_rn(index_frac, static_cast<double>(offset));
+  float y = wing<FMT, CH>(0.0f, tab, offset, index_step, (nwin - offset) / index_step, eta, frames, n - first_in, -1, n_in);
+  index_frac = __dmul_rn(__dsub_rn(scale, frac), static_cast<double>(num_table));
+  offset = static_cast<int>(index_frac);
+  eta = __dsub_rn(index_frac, static_cast<double>(offset));
+  y = wing<FMT, CH>(y, tab, offset, index_step, (nwin - offset) / index_step, eta, frames, n + 1 - first_in, 1, n_in);
+  out[o] = y;
+}
+
 }  // namespace
 
 struct lspa_ctx {
@@ -161,6 +239,10 @@ struct lspa_ctx {
   float2* d_tw = nullptr;
   float* d_hann = nullptr;
   float* d_basis = nullptr;    // [kMaxMels, kBins]
+  // the resampling filter: 0 entries until one is loaded
+  int nwin = 0, num_table = 0, index_step = 0;
+  double scale = 0.0;
+  double2* d_rs_tab = nullptr; // [nwin] (win, delta)
 };
 
 extern "C" {
@@ -174,6 +256,7 @@ int lspa_destroy(lspa_handle h) {
     if (h->d_tw) cudaFree(h->d_tw);
     if (h->d_hann) cudaFree(h->d_hann);
     if (h->d_basis) cudaFree(h->d_basis);
+    if (h->d_rs_tab) cudaFree(h->d_rs_tab);
   }
   delete h;
   return LSPG_OK;
@@ -247,6 +330,98 @@ int lspa_logmel_at(lspa_handle h, const float* audio, int64_t first_sample, int6
       audio, first_sample, n_samples, first_window, n_windows, frame_len, step, h->d_tw, h->d_hann, h->d_basis, h->n_mels,
       normalize ? 1 : 0, out);
   CUDA_TRY(cudaGetLastError());
+  return LSPG_OK;
+}
+
+int lspa_load_resample_filter(lspa_handle h, const double* win, const double* delta, int nwin, int num_table,
+                              double sample_ratio) {
+  if (!h || !win || !delta) return fail(LSPG_EINVAL, "null argument");
+  if (nwin < 2) return fail(LSPG_EINVAL, "nwin must be >= 2 (got %d)", nwin);
+  if (num_table < 1) return fail(LSPG_EINVAL, "num_table must be >= 1 (got %d)", num_table);
+  if (!(sample_ratio > 0.0) || !(sample_ratio < 1.0e6))
+    return fail(LSPG_EINVAL, "sample_ratio must be in (0, 1e6) (got %g)", sample_ratio);
+  const double scale = sample_ratio < 1.0 ? sample_ratio : 1.0;
+  const int index_step = static_cast<int>(scale * num_table);
+  if (index_step < 1)
+    return fail(LSPG_EINVAL, "int(min(1, sample_ratio) * num_table) must be >= 1 (got %g * %d)", scale, num_table);
+  if (int rc = capi::require_device<Lspa>(h->device, "lspa_load_resample_filter")) return rc;
+  DeviceGuard g(h->device);
+  h->nwin = 0;                                 // not usable until the copy is complete
+  if (h->d_rs_tab) cudaFree(h->d_rs_tab);
+  h->d_rs_tab = nullptr;
+  double2* tab = new double2[nwin];
+  for (int j = 0; j < nwin; ++j) tab[j] = make_double2(win[j], delta[j]);
+  cudaError_t e = cudaMalloc(&h->d_rs_tab, sizeof(double2) * nwin);
+  if (e == cudaSuccess) e = cudaMemcpy(h->d_rs_tab, tab, sizeof(double2) * nwin, cudaMemcpyHostToDevice);
+  delete[] tab;
+  if (e != cudaSuccess) return fail(LSPG_ECUDA, "lspa_load_resample_filter: %s", cudaGetErrorString(e));
+  h->num_table = num_table;
+  h->index_step = index_step;
+  h->scale = scale;
+  h->nwin = nwin;
+  return LSPG_OK;
+}
+
+int lspa_resample_at(lspa_handle h, const void* frames, int format, int channels, int64_t first_in, int64_t n_in,
+                     int64_t first_out, int64_t n_out, const int64_t* reg_table, int n_reg, float* out, void* stream) {
+  if (!h) return fail(LSPG_EINVAL, "null handle");
+  if (format != LSPA_FMT_F32 && format != LSPA_FMT_S16) return fail(LSPG_EINVAL, "unknown sample format %d", format);
+  if (channels != 1 && channels != 2) return fail(LSPG_EINVAL, "channels must be 1 or 2 (got %d)", channels);
+  if (n_in < 0 || n_out < 0 || first_in < 0 || first_out < 0)
+    return fail(LSPG_EINVAL, "first_in, n_in, first_out and n_out must be >= 0 (got %lld, %lld, %lld, %lld)",
+                static_cast<long long>(first_in), static_cast<long long>(n_in), static_cast<long long>(first_out),
+                static_cast<long long>(n_out));
+  if (n_in > (INT64_MAX >> 2) || n_out > (INT64_MAX >> 2) || first_out > (INT64_MAX >> 2))
+    return fail(LSPG_EINVAL, "counts must be below 2^61");
+  if ((!frames && n_in > 0) || (!out && n_out > 0) || !reg_table) return fail(LSPG_EINVAL, "null buffer");
+  if (n_reg < 2) return fail(LSPG_EINVAL, "the register table needs a row and the end row (got %d rows)", n_reg);
+  const int64_t(*reg)[4] = reinterpret_cast<const int64_t(*)[4]>(reg_table);
+  if (reg[0][0] != 0) return fail(LSPG_EINVAL, "the register table must start at output 0");
+  for (int i = 0; i + 1 < n_reg; ++i) {
+    if (reg[i + 1][0] <= reg[i][0]) return fail(LSPG_EINVAL, "register rows must start at increasing outputs (row %d)", i + 1);
+    if (reg[i][1] < 0 || reg[i][2] < 0 || reg[i][3] < -1022 || reg[i][3] > 1023 ||
+        reg[i][1] + (reg[i + 1][0] - 1 - reg[i][0]) * static_cast<double>(reg[i][2]) >= 9007199254740992.0)
+      return fail(LSPG_EINVAL, "register row %d is out of range", i);
+  }
+  if (first_out + n_out > reg[n_reg - 1][0])
+    return fail(LSPG_EINVAL, "outputs up to %lld requested, the register table ends at %lld",
+                static_cast<long long>(first_out + n_out), static_cast<long long>(reg[n_reg - 1][0]));
+  if (int rc = capi::require_device<Lspa>(h->device, "lspa_resample_at")) return rc;
+  if (h->nwin == 0) return fail(LSPG_ESTATE, "lspa_load_resample_filter has not been called");
+  if (n_out == 0) return LSPG_OK;
+  int r = 0;
+  while (r + 2 < n_reg && reg[r + 1][0] <= first_out) ++r;
+  if (first_in > 0) {                          // the left wing of output first_out reads back to n - (nwin / step - 1)
+    const int64_t n0 = static_cast<int64_t>(std::ldexp(static_cast<double>(reg[r][1] + (first_out - reg[r][0]) * reg[r][2]),
+                                                       static_cast<int>(reg[r][3])));
+    if (n0 - (h->nwin / h->index_step - 1) < first_in)
+      return fail(LSPG_EINVAL, "output %lld reads input frames from %lld, before the first frame given (%lld)",
+                  static_cast<long long>(first_out), static_cast<long long>(n0 - (h->nwin / h->index_step - 1)),
+                  static_cast<long long>(first_in));
+  }
+  DeviceGuard g(h->device);
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  for (int64_t t = first_out, end = first_out + n_out; t < end;) {       // one launch per kMaxRegRows register rows
+    while (r + 2 < n_reg && reg[r + 1][0] <= t) ++r;
+    RegRows rows;
+    rows.n = 0;
+    for (int i = r; i < n_reg - 1 && rows.n < kMaxRegRows; ++i, ++rows.n) {
+      rows.t0[rows.n] = reg[i][0];
+      rows.base[rows.n] = reg[i][1];
+      rows.k[rows.n] = reg[i][2];
+      rows.e[rows.n] = static_cast<int>(reg[i][3]);
+    }
+    const int64_t stop = std::min(end, reg[r + rows.n][0]);
+    const int64_t m = stop - t;
+    const int64_t blocks = (m + kRsThreads - 1) / kRsThreads;
+    if (blocks > INT32_MAX) return fail(LSPG_EINVAL, "too many outputs in one call (%lld)", static_cast<long long>(m));
+    auto kern = format == LSPA_FMT_S16 ? (channels == 1 ? lspa_resample_kernel<LSPA_FMT_S16, 1> : lspa_resample_kernel<LSPA_FMT_S16, 2>)
+                                       : (channels == 1 ? lspa_resample_kernel<LSPA_FMT_F32, 1> : lspa_resample_kernel<LSPA_FMT_F32, 2>);
+    kern<<<static_cast<unsigned>(blocks), kRsThreads, 0, st>>>(frames, first_in, n_in, t, m, rows, h->d_rs_tab, h->nwin,
+                                                                h->num_table, h->index_step, h->scale, out + (t - first_out));
+    CUDA_TRY(cudaGetLastError());
+    t = stop;
+  }
   return LSPG_OK;
 }
 

@@ -13,10 +13,15 @@ The look-ahead is the models': Audio2Mouth's ``frame_future`` (18) and Audio2Hea
 ``PortraitStream`` goes on to frames: the track rows through stage 5 (``LandmarkPostprocessor.stream``, which adds the
 smoothing radii to the look-ahead: frame t needs head-pose row t + max(rr, rt), so for May's settings APC pair t + 55),
 then the rasteriser and the generator, one frame per generator call.
+
+Both streams take 16 kHz mono samples, or native-rate frames through an ``audio.Resampler`` (``AudioStream(...,
+resampler=...)``): librosa.load's mono mix and resampling, streamed bit for bit, with ``resample_counts`` frames of
+look-ahead in front (about 4 ms at 48 kHz).
 """
 from __future__ import annotations
 
 import dataclasses
+import math
 from typing import NamedTuple, Optional
 
 import torch
@@ -40,6 +45,31 @@ def mel_windows(n_samples: int, finished: bool, frame_len: int = 266, step: floa
     while int(i * step) + frame_len <= n_samples:
         i += 1
     return min(i, total)
+
+
+def resample_counts(n_in: int, finished: bool, orig_sr: int, res_type: str = "kaiser_best", sr: int = SR) -> int:
+    """16 kHz samples ready after ``n_in`` native-rate frames (``audio.ResampleStream``).  Output t reads input frames
+    up to n + nwin // index_step, n = int(register(t)) (the right wing's longest reach), so it is ready once those are
+    in and t < int(n_in * ratio) (resampy's count, monotone in n_in).  At the end of the clip all ``ceil(n_in * ratio)``
+    (``fix_length``'s zero included), or 0 where resampy refuses the clip.  At ``orig_sr == sr`` every frame, at once."""
+    if orig_sr == sr:
+        return n_in
+    from .audio import filter_shape, register_at, register_table
+    ratio = float(sr) / orig_sr
+    total = int(n_in * ratio)
+    if finished:
+        return int(math.ceil(n_in * ratio)) if total >= 1 else 0
+    nwin, _, index_step = filter_shape(orig_sr, res_type, sr)
+    last = n_in - 1 - nwin // index_step                 # the last frame an output may read from its window's centre
+    if last < 0:
+        return 0
+    reg = register_table(ratio)
+    t = max(0, int(last * ratio))                        # near the count; the fp64 registers decide
+    while t > 0 and int(register_at(reg, t - 1)) > last:
+        t -= 1
+    while int(register_at(reg, t)) <= last:
+        t += 1
+    return min(t, total)
 
 
 class Counts(NamedTuple):
@@ -96,7 +126,9 @@ class AudioStream:
     return ``StreamRows``.  The concatenated tracks equal ``mouth.generate(blend)`` and
     ``headpose.generate(blend.view(-1, 2 * APC_hidden), pre_headpose, noise, sigma_scale)`` of the whole clip, with
     ``blend = projector.project_features(apc.forward(mel.logmel(audio)), k, percent)`` (or the APC features without a
-    projector), bit for bit.  ``noise`` is as for ``HeadposeGenerator.stream``: None draws from torch's global CPU
+    projector), bit for bit.  With ``resampler`` (an ``audio.Resampler``) ``push`` takes native-rate frames and the
+    audio is ``resampler.resample`` of them, streamed (``ResampleStream``); the counts are then ``ready_counts`` of
+    ``resample_counts``.  ``noise`` is as for ``HeadposeGenerator.stream``: None draws from torch's global CPU
     generator frame by frame, in the order the whole-clip draw takes.
 
     Device memory does not grow with the stream: the audio tail of the next window, one APC row waiting for its pair, the
@@ -105,7 +137,9 @@ class AudioStream:
     All pushes of a session go on one CUDA stream (the current one when ``push`` is called)."""
 
     def __init__(self, mel, apc, mouth, headpose, projector=None, k: int = 10, percent: float = 1.0, pre_headpose=None,
-                 sigma_scale: float = 0.3, noise=None, winlen: float = 1 / 60, winstep: float = 0.5 / 60, sr: int = SR):
+                 sigma_scale: float = 0.3, noise=None, winlen: float = 1 / 60, winstep: float = 0.5 / 60, sr: int = SR,
+                 resampler=None):
+        self._rs = resampler.stream() if resampler is not None else None
         self._mel = mel.stream(winlen, winstep, sr)
         self._apc = apc.stream()
         self._mouth = mouth.stream()
@@ -119,12 +153,16 @@ class AudioStream:
     def push(self, samples) -> StreamRows:
         if self.finished:
             raise RuntimeError("the stream has finished")
+        if self._rs is not None:
+            samples = self._rs.push(samples)
         return self._step(self._mel.push(samples), False)
 
     def finish(self) -> StreamRows:
         if self.finished:
             raise RuntimeError("the stream has finished")
         self.finished = True
+        if self._rs is not None:
+            return self._step(torch.cat([self._mel.push(self._rs.finish()), self._mel.finish()]), True)
         return self._step(self._mel.finish(), True)
 
     def _step(self, mel: torch.Tensor, finished: bool) -> StreamRows:
@@ -164,7 +202,7 @@ class PortraitFrames:
 class PortraitStream:
     """Live audio to portrait frames: ``AudioStream`` (stages 1-4) -> ``LandmarkStream`` (stage 5) ->
     ``net.draw_feature_maps`` -> ``net.render_image`` (stage 6).  ``push(samples)`` / ``finish()`` return
-    ``PortraitFrames``; how many is ``portrait_counts``.
+    ``PortraitFrames``; how many is ``portrait_counts`` (of ``resample_counts`` when the audio stream resamples).
 
     ``audio_stream`` is a fresh ``AudioStream``; ``post`` a ``LandmarkPostprocessor``, ``params`` its ``StageParams``;
     ``net`` the ``Feature2Face_G`` and ``cand`` its candidate images ``[1, 3 k, H, W]`` on the device.  The landmarks
