@@ -59,7 +59,10 @@ int lsph_load_weights(lsph_handle h, const lspg_tensor* tensors, int n);
  * the shipped options) - then 32 floats holding the network input of the next step (the last sample). */
 int lsph_state_bytes(lsph_handle h, size_t* bytes);
 
-/* Bytes of device workspace lsph_generate_stream needs for n_audio audio rows. */
+/* Bytes of device workspace lsph_generate_stream needs for n_audio audio rows.  After a call the workspace holds, as fp32
+ * arrays each padded to a multiple of 64 floats, in this order: ds1 [n_audio][apc_hidden] (audio_downsample's first
+ * Linear, BatchNorm and LeakyReLU), ds2 [n_audio][apc_hidden] (its second Linear) and cond
+ * [n_audio][layers*blocks][2*residual_ch] (each block's cond filter then cond gate projection plus both biases). */
 int lsph_stream_workspace_bytes(lsph_handle h, int n_audio, size_t* bytes);
 
 /* Replaces Audio2HeadposeModel.generate_sequences (models/audio2headpose_model.py:133-187; WaveNet decoder,

@@ -22,6 +22,7 @@ def lrelu(x):
 
 def generate_incremental(sd, audio_feats, pre_headpose, noise, opt, sigma_scale=0.3, return_params=False):
     f64 = lambda k: sd[k].double().numpy()      # noqa: E731  float64 emulation: isolates algorithmic equivalence from rounding
+    bias = lambda k, n: f64(k) if k in sd else np.zeros(n)     # noqa: E731  conv biases are absent when use_bias is off
     ff, rf = opt.frame_future, opt.A2H_receptive_field
     ndim, nc = opt.A2H_GMM_ndim, opt.A2H_GMM_ncenter
     audio = np.asarray(audio_feats, np.float64).reshape(-1, 2 * opt.APC_hidden_size)
@@ -42,9 +43,10 @@ def generate_incremental(sd, audio_feats, pre_headpose, noise, opt, sigma_scale=
     blk = []
     for i in range(nl):
         p = f"WaveNet.residual_blocks.{i}."
-        blk.append(dict(Wf=f64(p + "filter_conv.weight"), bf=f64(p + "filter_conv.bias"), Wg=f64(p + "gate_conv.weight"),
-                        bg=f64(p + "gate_conv.bias"), Wr=f64(p + "residual_conv.weight")[:, :, 0], br=f64(p + "residual_conv.bias"),
-                        Ws=f64(p + "skip_conv.weight")[:, :, 0], bs=f64(p + "skip_conv.bias")))
+        R_, S_ = opt.A2H_wavenet_residual_channels, opt.A2H_wavenet_skip_channels
+        blk.append(dict(Wf=f64(p + "filter_conv.weight"), bf=bias(p + "filter_conv.bias", R_), Wg=f64(p + "gate_conv.weight"),
+                        bg=bias(p + "gate_conv.bias", R_), Wr=f64(p + "residual_conv.weight")[:, :, 0], br=bias(p + "residual_conv.bias", R_),
+                        Ws=f64(p + "skip_conv.weight")[:, :, 0], bs=bias(p + "skip_conv.bias", S_)))
     T = rf - 1 + nframe
     R = opt.A2H_wavenet_residual_channels
     X = np.zeros((nl, T, R))                        # input of block l at absolute time t
