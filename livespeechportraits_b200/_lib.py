@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h and include/lspr.h.  Plain pointers and sizes only."""
+"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h, include/lspr.h and include/lspj.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
 import contextlib
@@ -137,11 +137,18 @@ ARGTYPES = {
     "lspr_debug_packed": [_p, _i, _p, _pi64],
     "lspr_destroy": [_p],
     "lspr_last_error": [],
+    # include/lspj.h (baseline JPEG encoder, demo.py's JPEG boundary)
+    "lspj_create": [_out_handle, _i],
+    "lspj_max_bytes": [_p, _i, _i, _i, _psz],
+    "lspj_workspace_bytes": [_p, _i, _i, _i, _i, _psz],
+    "lspj_encode": [_p, _p, _i, _i, _i, _i, _i, _p, _i64, _p, _p, _sz, _p],
+    "lspj_destroy": [_p],
+    "lspj_last_error": [],
 }
 
 
 def symbols(prefix: Optional[str] = None) -> List[str]:
-    """The bound symbols of one module (``"lspm"``, ...), or of all six."""
+    """The bound symbols of one module (``"lspm"``, ...), or of all seven."""
     return [name for name in ARGTYPES if prefix is None or name.startswith(prefix + "_")]
 
 

@@ -1,7 +1,7 @@
 """Compile the CUDA extension in-tree for sm_90a (nvcc cross-compiles without a GPU).
 
 ``python -m livespeechportraits_b200.build`` or ``build_library()`` produces
-``livespeechportraits_b200/liblspg.so`` - a plain C-ABI shared library (include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h, include/lspr.h), statically linked
+``livespeechportraits_b200/liblspg.so`` - a plain C-ABI shared library (include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h, include/lspr.h, include/lspj.h), statically linked
 against cudart and without a link-time dependency on libcuda (the one driver entry point it needs,
 cuTensorMapEncodeTiled, is resolved at run time), so it also loads on a machine without a driver.
 """
@@ -15,11 +15,11 @@ import sys
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "liblspg.so")
-SOURCES = ["lspg.cu", "lsph.cu", "lspm.cu", "lspa.cu", "lspl.cu", "lspr.cu"]
+SOURCES = ["lspg.cu", "lsph.cu", "lspm.cu", "lspa.cu", "lspl.cu", "lspr.cu", "lspj.cu"]
 HEADERS = ["capi.cuh", "conv_wgmma.cuh", "ptx.cuh", "aux_kernels.cuh", "raster.cuh", "gemm_nt.cuh", os.path.join("..", "..", "include", "lspg.h"),
            os.path.join("..", "..", "include", "lsph.h"), os.path.join("..", "..", "include", "lspm.h"),
            os.path.join("..", "..", "include", "lspa.h"), os.path.join("..", "..", "include", "lspl.h"),
-           os.path.join("..", "..", "include", "lspr.h")]
+           os.path.join("..", "..", "include", "lspr.h"), os.path.join("..", "..", "include", "lspj.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
