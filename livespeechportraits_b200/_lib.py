@@ -1,4 +1,4 @@
-"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h, include/lspr.h and include/lspj.h.  Plain pointers and sizes only."""
+"""ctypes binding of the C ABI in include/lspg.h, include/lsph.h, include/lspm.h, include/lspa.h, include/lspl.h, include/lspr.h, include/lspj.h and include/lspv.h.  Plain pointers and sizes only."""
 from __future__ import annotations
 
 import contextlib
@@ -144,11 +144,19 @@ ARGTYPES = {
     "lspj_encode": [_p, _p, _i, _i, _i, _i, _i, _p, _i64, _p, _p, _sz, _p],
     "lspj_destroy": [_p],
     "lspj_last_error": [],
+    # include/lspv.h (H.264 Constrained Baseline encoder)
+    "lspv_create": [_out_handle, _i, _i, _i, _i, _i],
+    "lspv_max_bytes": [_p, _i, _i, _psz],
+    "lspv_state_bytes": [_p, _i, _i, _psz],
+    "lspv_workspace_bytes": [_p, _i, _i, _psz],
+    "lspv_encode": [_p, _p, _i, _i, _i, _i, _i64, _p, _p, _i64, _p, _p, _p, _sz, _p],
+    "lspv_destroy": [_p],
+    "lspv_last_error": [],
 }
 
 
 def symbols(prefix: Optional[str] = None) -> List[str]:
-    """The bound symbols of one module (``"lspm"``, ...), or of all seven."""
+    """The bound symbols of one module (``"lspm"``, ...), or of all eight."""
     return [name for name in ARGTYPES if prefix is None or name.startswith(prefix + "_")]
 
 

@@ -1,4 +1,4 @@
-// Host-side plumbing shared by the seven C-ABI modules (lspg, lsph, lspm, lspa, lspl, lspr, lspj): the per-module error
+// Host-side plumbing shared by the eight C-ABI modules (lspg, lsph, lspm, lspa, lspl, lspr, lspj, lspv): the per-module error
 // channel, device validation, the current-device guard and the state-dict table.  No device code.
 //
 // Each module binds the error channel to a tag type of its own in one line,

@@ -155,6 +155,9 @@ _KEYFRAME = 0x10
 class MjpegAviWriter:
     """A Motion-JPEG AVI file (fourcc ``MJPG``) with an optional audio stream, written without ffmpeg.
 
+    ``fourcc="H264"`` makes it an H.264 AVI instead: each frame is one Annex B access unit (``H264Encoder``), and only
+    frames written with ``keyframe=True`` (the IDRs) carry the keyframe flag in ``idx1`` and ``ix00``.
+
     ``write_frame(jpeg_bytes)`` appends one complete .jpg file as a frame; ``write_audio(samples)`` appends audio: numpy
     ``[n]`` or ``[n, channels]`` samples, float32 (``audio_format="f32"``, WAVE_FORMAT_IEEE_FLOAT, what demo.py's
     ``write_wav`` + ``ffmpeg -codec copy`` puts in its .avi) or int16 (``"s16"``, PCM).  Audio is written in chunks after
@@ -164,7 +167,10 @@ class MjpegAviWriter:
     the 1 GB of AVI 1.0 stay readable."""
 
     def __init__(self, path: str, size, fps: float = 60, audio_rate: Optional[int] = None, audio_channels: int = 1,
-                 audio_format: str = "f32", segment_bytes: int = 1 << 30):
+                 audio_format: str = "f32", segment_bytes: int = 1 << 30, fourcc: str = "MJPG"):
+        if fourcc not in ("MJPG", "H264"):
+            raise ValueError(f"fourcc must be 'MJPG' or 'H264' (got {fourcc!r})")
+        self.fourcc = fourcc.encode()
         if audio_format not in ("f32", "s16"):
             raise ValueError(f"audio_format must be 'f32' or 's16' (got {audio_format!r})")
         if audio_channels not in (1, 2):
@@ -206,7 +212,7 @@ class MjpegAviWriter:
             self._strh.append(f.tell() + 8)
             f.write(b"strh" + struct.pack("<I", 56) + bytes(56))
             if s == 0:
-                f.write(b"strf" + struct.pack("<IIiiHH4sIiiII", 40, 40, self.width, self.height, 1, 24, b"MJPG",
+                f.write(b"strf" + struct.pack("<IIiiHH4sIiiII", 40, 40, self.width, self.height, 1, 24, self.fourcc,
                                               self.width * self.height * 3, 0, 0, 0, 0))
             else:
                 fmt = 3 if self.dtype == np.float32 else 1
@@ -238,7 +244,7 @@ class MjpegAviWriter:
             self._riff = 0
         self._movi = f.tell()
         f.write(b"LIST\0\0\0\0movi")
-        self._chunks: List[List[tuple]] = [[], []]     # per stream: (data offset, size, duration)
+        self._chunks: List[List[tuple]] = [[], []]     # per stream: (data offset, size, duration, keyframe)
         self._first = first
 
     def _close_segment(self):
@@ -252,19 +258,19 @@ class MjpegAviWriter:
             cid = b"00dc" if s == 0 else b"01wb"
             f.write((b"ix00" if s == 0 else b"ix01") + struct.pack("<IHBBI4sQI", 24 + 8 * len(chunks), 2, 0, 1, len(chunks),
                                                                       cid, base, 0))
-            f.write(b"".join(struct.pack("<II", off - base, size) for off, size, _ in chunks))
-            self._segments[s].append((at, 32 + 8 * len(chunks), sum(d for _, _, d in chunks)))
+            f.write(b"".join(struct.pack("<II", off - base, size | (0 if key else 1 << 31)) for off, size, _, key in chunks))
+            self._segments[s].append((at, 32 + 8 * len(chunks), sum(c[2] for c in chunks)))
             if len(self._segments[s]) > _SUPER_ENTRIES:
                 raise RuntimeError(f"more than {_SUPER_ENTRIES} RIFF segments; raise segment_bytes")
         self._patch_size(self._movi)
         if self._first:
             f.write(b"idx1" + struct.pack("<I", 16 * len(self._idx1)))
-            f.write(b"".join(struct.pack("<4sIII", cid, _KEYFRAME, off - self._movi - 8, size)
-                             for cid, off, size in self._idx1))
+            f.write(b"".join(struct.pack("<4sIII", cid, _KEYFRAME if key else 0, off - self._movi - 8, size)
+                             for cid, off, size, key in self._idx1))
             self._first_frames = self.frames
         self._patch_size(self._riff)
 
-    def _chunk(self, stream: int, data: bytes, duration: int):
+    def _chunk(self, stream: int, data: bytes, duration: int, key: bool = True):
         size = len(data)
         need = 8 + size + (size & 1) + 8 * 8 + 64            # the chunk and room for its index entries
         if self._first:
@@ -275,14 +281,14 @@ class MjpegAviWriter:
         cid = b"00dc" if stream == 0 else b"01wb"
         at = self._f.tell()
         self._f.write(cid + struct.pack("<I", size) + data + (b"\0" if size & 1 else b""))
-        self._chunks[stream].append((at + 8, size, duration))
+        self._chunks[stream].append((at + 8, size, duration, key))
         if self._first:
-            self._idx1.append((cid, at, size))
+            self._idx1.append((cid, at, size, key))
         self._max_chunk = max(self._max_chunk, size)
 
     # -- public -----------------------------------------------------------------------------------------------------
-    def write_frame(self, jpeg: bytes) -> None:
-        self._chunk(0, bytes(jpeg), 1)
+    def write_frame(self, jpeg: bytes, keyframe: bool = True) -> None:
+        self._chunk(0, bytes(jpeg), 1, bool(keyframe))
         self.frames += 1
         if self.audio_rate is not None:
             self._flush_audio(self._audio_end(self.frames))
@@ -331,7 +337,7 @@ class MjpegAviWriter:
         for s in range(self._streams):
             f.seek(self._strh[s])
             if s == 0:
-                f.write(struct.pack("<4s4sIHHIIIIIIiIhhhh", b"vids", b"MJPG", 0, 0, 0, 0, scale, rate, 0, self.frames,
+                f.write(struct.pack("<4s4sIHHIIIIIIiIhhhh", b"vids", self.fourcc, 0, 0, 0, 0, scale, rate, 0, self.frames,
                                     self._max_chunk, -1, 0, 0, 0, self.width, self.height))
             else:
                 f.write(struct.pack("<4s4sIHHIIIIIIiIhhhh", b"auds", b"\0\0\0\0", 0, 0, 0, 0, self.block_align,
@@ -384,10 +390,11 @@ class _JpegSink:
                 item = self.q.get()
                 if item is None:
                     return
-                ev, data, sizes_host, n, audio, release = item
+                ev, data, sizes_host, n, audio, release, keys_host = item
                 self._wait(ev)
                 t0 = time.perf_counter()
                 sizes = sizes_host[:n].tolist()
+                keys = [True] * n if keys_host is None else [bool(k) for k in keys_host[:n].tolist()]
                 host = torch.empty(max(sum(sizes), 1), dtype=torch.uint8, pin_memory=True)
                 with torch.cuda.stream(self.copy_stream):
                     self.copy_stream.wait_event(ev)
@@ -403,23 +410,23 @@ class _JpegSink:
                 if audio is not None and self.writer is not None:
                     self.writer.write_audio(audio)    # buffered; each frame below flushes the audio of its interval
                 buf, at = host.numpy(), 0
-                for sz in sizes:
+                for sz, key in zip(sizes, keys):
                     jpg = buf[at:at + sz].tobytes()
                     at += sz
                     if self.frames_dir is not None:
                         with open(os.path.join(self.frames_dir, f"{self.prefix}{self.frames + 1}.jpg"), "wb") as f:
                             f.write(jpg)
                     if self.writer is not None:
-                        self.writer.write_frame(jpg)
+                        self.writer.write_frame(jpg, key)
                     self.frames += 1
                 self.busy_seconds += time.perf_counter() - t0
         except BaseException as exc:      # noqa: BLE001 - surfaced by close()
             self.error = exc
 
-    def put(self, ev, data, sizes_host, n, audio=None, release=None) -> None:
+    def put(self, ev, data, sizes_host, n, audio=None, release=None, keys_host=None) -> None:
         if self.error is not None:
             raise self.error
-        self.q.put((ev, data, sizes_host, n, audio, release))
+        self.q.put((ev, data, sizes_host, n, audio, release, keys_host))
 
     def close(self) -> None:
         self.q.put(None)
@@ -431,24 +438,35 @@ class _JpegSink:
 
 
 def _encode_and_queue(enc, images, slot, sink, audio=None):
-    """Encodes ``images`` into the slot's device buffers on the current stream, copies ``sizes`` into the slot's pinned
-    buffer behind it, records an event and queues the batch for ``sink``."""
+    """Encodes ``images`` into the slot's device buffers on the current stream, copies ``sizes`` (and for an
+    ``H264Stream`` the IDR flags) into the slot's pinned buffers behind it, records an event and queues the batch for
+    ``sink``.  ``enc`` is a ``JpegEncoder`` or an ``H264Stream``."""
+    from .h264 import H264Stream
+    h264 = isinstance(enc, H264Stream)
     n = images.shape[0]
     h, w = int(images.shape[1]), int(images.shape[2])
     c = 3 if images.dim() == 4 else 1
     dev = images.device
-    stride = enc.max_bytes(h, w, c)
+    stride = enc.encoder.max_bytes(h, w) if h264 else enc.max_bytes(h, w, c)
     if slot.get("data") is None or slot["data"].shape[0] < n or slot["data"].shape[1] != stride:
         slot["data"] = torch.empty((max(n, 1), stride), dtype=torch.uint8, device=dev)
         slot["sizes"] = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
         slot["sizes_host"] = torch.empty(max(n, 1), dtype=torch.int32, pin_memory=True)
-    slot["ws"] = _lib.reserve(slot.get("ws"), enc.workspace_bytes(n, h, w, c), dev)
+        if h264:
+            slot["idr"] = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+            slot["idr_host"] = torch.empty(max(n, 1), dtype=torch.uint8, pin_memory=True)
+    if not h264:
+        slot["ws"] = _lib.reserve(slot.get("ws"), enc.workspace_bytes(n, h, w, c), dev)
     if n:
-        batch = enc.encode_into(images, slot["data"], slot["sizes"], slot["ws"])
+        if h264:
+            batch = enc.push_into(images, slot["data"], slot["sizes"], slot["idr"])
+            slot["idr_host"][:n].copy_(batch.is_idr, non_blocking=True)
+        else:
+            batch = enc.encode_into(images, slot["data"], slot["sizes"], slot["ws"])
         slot["sizes_host"][:n].copy_(batch.sizes, non_blocking=True)
     ev = torch.cuda.Event()
     ev.record(torch.cuda.current_stream(dev))
-    sink.put(ev, slot["data"], slot["sizes_host"], n, audio, slot.get("free"))
+    sink.put(ev, slot["data"], slot["sizes_host"], n, audio, slot.get("free"), slot.get("idr_host") if h264 else None)
 
 
 def render_to_mjpeg(net, landmarks, shoulders, cand, output_path: str, size: tuple = (512, 512), fps: float = 60,
@@ -465,6 +483,28 @@ def render_to_mjpeg(net, landmarks, shoulders, cand, output_path: str, size: tup
     ``frames_dir``: also write ``pred_<j+1>.jpg`` (and ``input_<j+1>.jpg`` for the maps) with demo.py's bytes.
     Returns ``{"frames", "seconds", "encode_seconds", "writer", "bytes"}``."""
     from .jpeg import JpegEncoder
+    enc = JpegEncoder(cand.device, quality)
+    return _render_to_avi(net, landmarks, shoulders, cand, output_path, size, fps, batch, audio, audio_rate,
+                          feature_maps_path, frames_dir, precision, "MJPG", lambda: enc, f"MJPG q{quality}")
+
+
+def render_to_h264(net, landmarks, shoulders, cand, output_path: str, size: tuple = (512, 512), fps: float = 60,
+                   batch: int = 32, qp: int = 26, gop: int = 60, search: int = 16, audio=None, audio_rate: int = 16000,
+                   feature_maps_path: Optional[str] = None, precision: Optional[str] = None) -> dict:
+    """``render_to_mjpeg`` with H.264 video: the frames are encoded on the compute stream by ``H264Encoder`` (fixed
+    ``qp``, an IDR every ``gop`` frames, full-pel motion within ``search``) and the AVI (fourcc ``H264``) holds one
+    access unit per frame, keyframe-flagged on the IDRs.  ``feature_maps_path``: the maps as a second H.264 AVI of the
+    grey ``np.uint8(map * 255)`` frames.  Returns ``{"frames", "seconds", "encode_seconds", "writer", "bytes"}``."""
+    from .h264 import H264Encoder
+    enc = H264Encoder(cand.device, qp=qp, gop=gop, search=search, fps=int(round(fps)))
+    return _render_to_avi(net, landmarks, shoulders, cand, output_path, size, fps, batch, audio, audio_rate,
+                          feature_maps_path, None, precision, "H264", enc.stream, f"H264 qp{qp} gop{gop}")
+
+
+def _render_to_avi(net, landmarks, shoulders, cand, output_path, size, fps, batch, audio, audio_rate, feature_maps_path,
+                   frames_dir, precision, fourcc, make_encoder, label) -> dict:
+    """The body of ``render_to_mjpeg`` / ``render_to_h264``: ``make_encoder()`` gives the frames' encoder (and, called
+    again, the maps'): a ``JpegEncoder`` or an ``H264Stream``."""
     n = int(landmarks.shape[0])
     w, h = int(size[0]), int(size[1])
     dev = cand.device
@@ -474,15 +514,16 @@ def render_to_mjpeg(net, landmarks, shoulders, cand, output_path: str, size: tup
     channels = 1 if a is None or a.ndim == 1 else int(a.shape[1])
     t0 = time.perf_counter()
     writer = MjpegAviWriter(output_path, (w, h), fps, None if a is None else audio_rate, channels,
-                            "s16" if a is not None and a.dtype == np.int16 else "f32")
+                            "s16" if a is not None and a.dtype == np.int16 else "f32", fourcc=fourcc)
     if a is not None:
         writer.write_audio(a)                         # interleaved as the frames arrive, cut on close
     sink = _JpegSink(writer, dev, frames_dir, "pred_")
     fsink = None
     if feature_maps_path is not None or frames_dir is not None:
-        fwriter = None if feature_maps_path is None else MjpegAviWriter(feature_maps_path, (w, h), fps)
+        fwriter = None if feature_maps_path is None else MjpegAviWriter(feature_maps_path, (w, h), fps, fourcc=fourcc)
         fsink = _JpegSink(fwriter, dev, frames_dir, "input_")
-    enc = JpegEncoder(dev, quality)
+    enc = make_encoder()
+    fenc = None if fsink is None else make_encoder()
     compute = torch.cuda.Stream(dev)
     compute.wait_stream(torch.cuda.current_stream(dev))
     slots = [{"free": threading.Event()} for _ in range(2)]
@@ -502,7 +543,7 @@ def render_to_mjpeg(net, landmarks, shoulders, cand, output_path: str, size: tup
                 if fsink is not None:
                     fslot["free"].wait()
                     fslot["free"].clear()
-                    _encode_and_queue(enc, (fm[:ln, 0] * 255.0).to(torch.uint8), fslot, fsink)
+                    _encode_and_queue(fenc, (fm[:ln, 0] * 255.0).to(torch.uint8), fslot, fsink)
                 cd = cand[off:off + ln] if cand.shape[0] == n and n > 1 else cand[:1]
                 net.render(fm[:ln], cd, out=frames[:ln], precision=precision, _uint8=True)
                 _encode_and_queue(enc, frames[:ln], slot, sink)
@@ -512,11 +553,13 @@ def render_to_mjpeg(net, landmarks, shoulders, cand, output_path: str, size: tup
             fsink.close()
     torch.cuda.current_stream(dev).wait_stream(compute)
     return {"frames": n, "seconds": time.perf_counter() - t0, "encode_seconds": sink.busy_seconds,
-            "writer": f"MJPG q{quality} {fps:g} fps {w}x{h}", "bytes": os.path.getsize(output_path)}
+            "writer": f"{label} {fps:g} fps {w}x{h}", "bytes": os.path.getsize(output_path)}
 
 
 class PortraitRecorder:
-    """Records a ``PortraitStream`` into a Motion-JPEG AVI with its audio while it plays.
+    """Records a ``PortraitStream`` into a Motion-JPEG AVI with its audio while it plays (``codec="h264"``: an H.264 AVI,
+    the frames coded by ``H264Encoder`` at ``qp`` with an IDR every ``gop`` frames, the same stream a whole-clip encode
+    of the frames gives).
 
     ``push(samples)`` forwards to ``portrait_stream.push`` and returns its ``PortraitFrames`` unchanged; the frames are
     encoded on the same CUDA stream (``JpegEncoder``, PIL's bytes at ``quality``), and a writer thread waits for them,
@@ -528,11 +571,19 @@ class PortraitRecorder:
     _RING = 4                                          # pushes the writer thread may lag behind before push waits for it
 
     def __init__(self, portrait_stream, path: str, quality: int = 75, fps: float = 60, audio_rate: int = 16000,
-                 audio_channels: int = 1, audio_format: str = "f32"):
-        from .jpeg import JpegEncoder
+                 audio_channels: int = 1, audio_format: str = "f32", codec: str = "mjpeg", qp: int = 26, gop: int = 60):
+        if codec not in ("mjpeg", "h264"):
+            raise ValueError(f"codec must be 'mjpeg' or 'h264' (got {codec!r})")
         self.stream = portrait_stream
-        self._enc = JpegEncoder(portrait_stream._cand.device, quality)
-        self._dev = self._enc.device
+        if codec == "h264":
+            from .h264 import H264Encoder
+            self._enc = H264Encoder(portrait_stream._cand.device, qp=qp, gop=gop, fps=int(round(fps))).stream()
+            self._dev = self._enc.encoder.device
+        else:
+            from .jpeg import JpegEncoder
+            self._enc = JpegEncoder(portrait_stream._cand.device, quality)
+            self._dev = self._enc.device
+        self._fourcc = "H264" if codec == "h264" else "MJPG"
         self._path, self._fps = path, fps
         self._audio = (audio_rate, audio_channels, audio_format)
         self._dtype = np.float32 if audio_format == "f32" else np.int16
@@ -553,7 +604,8 @@ class PortraitRecorder:
     def _record(self, out, samples) -> None:
         if self._sink is None:
             w, h = self.stream._size
-            self._sink = _JpegSink(MjpegAviWriter(self._path, (w, h), self._fps, *self._audio), self._dev)
+            self._sink = _JpegSink(MjpegAviWriter(self._path, (w, h), self._fps, *self._audio, fourcc=self._fourcc),
+                                   self._dev)
         slot = self._slots[self._pushes % self._RING]
         self._pushes += 1
         slot["free"].wait()
