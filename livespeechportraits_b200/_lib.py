@@ -238,6 +238,16 @@ def reserve(buf: Optional[torch.Tensor], nbytes: int, device: torch.device) -> t
     return buf
 
 
+def frame_shape(images: torch.Tensor) -> Tuple[int, int, int, int]:
+    """``(n, H, W, components)`` of the frames the video encoders take: a uint8 CUDA tensor ``[n, H, W, 3]`` (RGB) or
+    ``[n, H, W]`` (grey)."""
+    if images.dtype != torch.uint8 or not images.is_cuda or images.dim() not in (3, 4) or \
+            (images.dim() == 4 and images.shape[3] != 3):
+        raise ValueError("images must be a uint8 CUDA tensor [n, H, W, 3] (RGB) or [n, H, W] (grey)")
+    n, h, w = images.shape[:3]
+    return int(n), int(h), int(w), 3 if images.dim() == 4 else 1
+
+
 def tensor_array(state_dict) -> Tuple[C.Array, list]:
     """A state dict as the ``lspg_tensor`` array of the ``*_load_weights`` calls: fp32 contiguous CPU copies, without
     BatchNorm's ``num_batches_tracked``.  The array points into ``keep``, which must outlive the call."""

@@ -16,7 +16,7 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "liblspg.so")
 SOURCES = ["lspg.cu", "lsph.cu", "lspm.cu", "lspa.cu", "lspl.cu", "lspr.cu", "lspj.cu", "lspv.cu"]
-HEADERS = ["capi.cuh", "conv_wgmma.cuh", "ptx.cuh", "aux_kernels.cuh", "raster.cuh", "gemm_nt.cuh", os.path.join("..", "..", "include", "lspg.h"),
+HEADERS = ["capi.cuh", "bitstream.cuh", "conv_wgmma.cuh", "ptx.cuh", "aux_kernels.cuh", "raster.cuh", "gemm_nt.cuh", os.path.join("..", "..", "include", "lspg.h"),
            os.path.join("..", "..", "include", "lsph.h"), os.path.join("..", "..", "include", "lspm.h"),
            os.path.join("..", "..", "include", "lspa.h"), os.path.join("..", "..", "include", "lspl.h"),
            os.path.join("..", "..", "include", "lspr.h"), os.path.join("..", "..", "include", "lspj.h"),

@@ -1,5 +1,5 @@
 // Host-side plumbing shared by the eight C-ABI modules (lspg, lsph, lspm, lspa, lspl, lspr, lspj, lspv): the per-module error
-// channel, device validation, the current-device guard and the state-dict table.  No device code.
+// channel, device validation, the current-device guard, workspace alignment and the state-dict table.  No device code.
 //
 // Each module binds the error channel to a tag type of its own in one line,
 //   struct Lspx;  constexpr auto fail = capi::fail<Lspx>;
@@ -60,6 +60,9 @@ int require_device(int device, const char* fn) {
   if (device >= 0) return LSPG_OK;
   return fail<Module>(LSPG_ENODEV, "host-only handle: %s needs an sm_90 device (no CPU path exists)", fn);
 }
+
+// x rounded up to a multiple of 256, the alignment of each region the modules carve out of a workspace.
+inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 // Makes `device` current for the scope and restores the caller's device when it ends, so no call leaves the calling
 // thread (and torch, which reads it back with cudaGetDevice) on the handle's device.  A host-only handle (device < 0)

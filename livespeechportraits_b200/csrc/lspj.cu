@@ -18,8 +18,13 @@
 #include <cstring>
 
 #include "../../include/lspj.h"
+#include "bitstream.cuh"
 #include "capi.cuh"
 
+using bitstream::block_exclusive_scan;
+using bitstream::BitWriter;
+using bitstream::Sum;
+using capi::align256;
 using capi::DeviceGuard;
 
 namespace {
@@ -277,35 +282,6 @@ __global__ void __launch_bounds__(kBlockThreads) lspj_block_kernel(const Params 
   frame_offs(p, f)[b] = bits;
 }
 
-// ---- block-wide exclusive scan -------------------------------------------------------------------------------------
-
-__device__ __forceinline__ uint32_t block_exclusive_scan(uint32_t v, uint32_t* total) {
-  __shared__ uint32_t warp_sums[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  uint32_t incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += t;
-  }
-  if (lane == 31) warp_sums[wid] = incl;
-  __syncthreads();
-  if (wid == 0) {
-    uint32_t s = lane < nw ? warp_sums[lane] : 0;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t t = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += t;
-    }
-    if (lane < nw) warp_sums[lane] = s;
-  }
-  __syncthreads();
-  const uint32_t excl = (wid ? warp_sums[wid - 1] : 0) + incl - v;
-  *total = warp_sums[nw - 1];
-  __syncthreads();                                          // warp_sums is reused by the next call
-  return excl;
-}
-
 // ---- 2. DC bits, bit offsets, zeroed bit buffer ---------------------------------------------------------------------
 
 __device__ __forceinline__ uint32_t dc_bits(const int16_t* coef, int b, int comps) {
@@ -320,44 +296,13 @@ __global__ void __launch_bounds__(kFrameThreads) lspj_offsets_kernel(const Param
   const int f = blockIdx.x;
   const int16_t* coef = frame_coef(p, f);
   uint32_t* offs = frame_offs(p, f);
-  const int per = (p.nblk + kFrameThreads - 1) / kFrameThreads;
-  const int b0 = min(p.nblk, static_cast<int>(threadIdx.x) * per), b1 = min(p.nblk, b0 + per);
-  uint32_t sum = 0;
-  for (int b = b0; b < b1; ++b) sum += offs[b] + dc_bits(coef, b, p.comps);
-  uint32_t total;
-  uint32_t at = block_exclusive_scan(sum, &total);
-  for (int b = b0; b < b1; ++b) {
-    const uint32_t bits = offs[b] + dc_bits(coef, b, p.comps);
-    offs[b] = at;
-    at += bits;
-  }
-  if (threadIdx.x == 0) offs[p.nblk] = total;
+  const uint32_t total = bitstream::counts_to_offsets(offs, p.nblk, 0u, [&](int b) { return dc_bits(coef, b, p.comps); });
   uint32_t* buf = frame_bits(p, f);
   const uint32_t words = (total + 31) / 32;
   for (uint32_t i = threadIdx.x; i < words; i += kFrameThreads) buf[i] = 0;
 }
 
 // ---- 3. Huffman coding ----------------------------------------------------------------------------------------------
-
-struct BitWriter {
-  uint32_t* buf;
-  uint32_t word;                // next word to write
-  int n;                        // bits held in acc (< 32 between puts)
-  uint64_t acc;
-
-  __device__ __forceinline__ void put(uint32_t code, int size) {
-    acc = (acc << size) | code;
-    n += size;
-    if (n >= 32) {
-      n -= 32;
-      atomicOr(buf + word++, static_cast<uint32_t>(acc >> n));
-      acc &= (uint64_t(1) << n) - 1;
-    }
-  }
-  __device__ __forceinline__ void flush() {
-    if (n > 0) atomicOr(buf + word, static_cast<uint32_t>(acc << (32 - n)));
-  }
-};
 
 __global__ void __launch_bounds__(kBlockThreads) lspj_pack_kernel(const Params p) {
   __shared__ uint32_t huff[4 * 256];
@@ -372,7 +317,7 @@ __global__ void __launch_bounds__(kBlockThreads) lspj_pack_kernel(const Params p
   const uint32_t* ac = huff + (chroma ? 3 : 1) * 256;
   const uint4* src = reinterpret_cast<const uint4*>(coef + static_cast<int64_t>(b) * 64);
   const int pb = prev_block(b, p.comps);
-  BitWriter w{frame_bits(p, f), off >> 5, static_cast<int>(off & 31), 0};
+  BitWriter w(frame_bits(p, f), off);
   {
     const int diff = coef[static_cast<int64_t>(b) * 64] - (pb >= 0 ? coef[static_cast<int64_t>(pb) * 64] : 0);
     const int n = nbits(diff);
@@ -432,7 +377,7 @@ __global__ void __launch_bounds__(kFrameThreads) lspj_stuff_kernel(const Params 
       }
     }
     uint32_t round_total;
-    uint32_t o = base + block_exclusive_scan(count, &round_total);
+    uint32_t o = base + block_exclusive_scan<Sum>(count, &round_total);
     if (at < nbytes) {
 #pragma unroll
       for (int i = 0; i < 16; ++i) {
@@ -504,8 +449,6 @@ int64_t max_bytes_of(int height, int width, int components) {
   const int64_t scan = (blocks_of(height, width, components) * kWorstBlockBits + 7) / 8;
   return header_bytes(hdr, height, width, components, 75) + 2 * scan + 2;
 }
-
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 FrameLayout layout_of(int height, int width, int components) {
   const size_t nblk = static_cast<size_t>(blocks_of(height, width, components));

@@ -30,6 +30,7 @@
 #include "../../include/lspl.h"
 #include "capi.cuh"
 
+using capi::align256;
 using capi::DeviceGuard;
 
 namespace {
@@ -93,20 +94,18 @@ struct LipState {
   long long count;
 };
 
-size_t align_up(size_t x) { return (x + 255) & ~size_t(255); }
-
 Workspace carve(void* base, int n, bool stream, size_t* total) {
   const int ctas = (n + kFrames - 1) / kFrames;
   size_t off = 0;
   Workspace w{};
   char* b = static_cast<char*>(base);
-  w.mouth = reinterpret_cast<double*>(b + off);   off = align_up(off + sizeof(double) * kMouthCols * size_t(n));
-  w.pose = reinterpret_cast<float*>(b + off);     off = align_up(off + sizeof(float) * 6 * size_t(n));
+  w.mouth = reinterpret_cast<double*>(b + off);   off = align256(off + sizeof(double) * kMouthCols * size_t(n));
+  w.pose = reinterpret_cast<float*>(b + off);     off = align256(off + sizeof(float) * 6 * size_t(n));
   if (stream) {
-    w.shift = reinterpret_cast<double*>(b + off); off = align_up(off + sizeof(double) * size_t(n));
+    w.shift = reinterpret_cast<double*>(b + off); off = align256(off + sizeof(double) * size_t(n));
   } else {
-    w.part_sum = reinterpret_cast<double*>(b + off); off = align_up(off + sizeof(double) * size_t(ctas));
-    w.part_cnt = reinterpret_cast<int*>(b + off);   off = align_up(off + sizeof(int) * size_t(ctas));
+    w.part_sum = reinterpret_cast<double*>(b + off); off = align256(off + sizeof(double) * size_t(ctas));
+    w.part_cnt = reinterpret_cast<int*>(b + off);   off = align256(off + sizeof(int) * size_t(ctas));
   }
   *total = off;
   return w;

@@ -24,6 +24,7 @@
 #include "../../include/lspm.h"
 #include "capi.cuh"
 
+using capi::align256;
 using capi::DeviceGuard;
 
 namespace {
@@ -343,7 +344,6 @@ __global__ void __launch_bounds__(kLleWarps * 32) lspm_lle_kernel(const float* _
 }
 
 int ceil_div(int a, int b) { return (a + b - 1) / b; }
-size_t align256(size_t b) { return (b + 255) & ~static_cast<size_t>(255); }
 
 // Database slices per query tile: fill kSMs x kKnnCtasPerSM CTAs once.  Depends on n only, so the workspace size does
 // not depend on the database; the launch uses min(this, number of 64-row tiles).

@@ -18,8 +18,14 @@
 #include <string>
 
 #include "../../include/lspv.h"
+#include "bitstream.cuh"
 #include "capi.cuh"
 
+using bitstream::block_exclusive_scan;
+using bitstream::BitWriter;
+using bitstream::Max;
+using bitstream::Sum;
+using capi::align256;
 using capi::DeviceGuard;
 
 namespace {
@@ -578,26 +584,6 @@ struct Counter {
   __device__ __forceinline__ void put(uint32_t, int size) { n += size; }
 };
 
-struct BitWriter {
-  uint32_t* buf;
-  uint32_t word;
-  int n;
-  uint64_t acc;
-  __device__ __forceinline__ void put(uint32_t code, int size) {   // size <= 32
-    if (!size) return;
-    acc = (acc << size) | code;
-    n += size;
-    if (n >= 32) {
-      n -= 32;
-      atomicOr(buf + word++, static_cast<uint32_t>(acc >> n));
-      acc &= (uint64_t(1) << n) - 1;
-    }
-  }
-  __device__ __forceinline__ void flush() {
-    if (n > 0) atomicOr(buf + word, static_cast<uint32_t>(acc << (32 - n)));
-  }
-};
-
 template <class W>
 __device__ __forceinline__ void put_ue(W& w, uint32_t v) {
   const int k = 32 - __clz(v + 1);
@@ -774,38 +760,6 @@ __global__ void __launch_bounds__(128) lspv_bits_kernel(const Params p) {
   mb_bits(p)[i] = c.n;
 }
 
-template <bool kMax>
-__device__ __forceinline__ int block_exclusive_scan(int v, int* total) {
-  __shared__ int warp_acc[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  auto op = [](int a, int b) { return kMax ? max(a, b) : a + b; };
-  const int ident = kMax ? -1 : 0;
-  int incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl = op(incl, u);
-  }
-  if (lane == 31) warp_acc[wid] = incl;
-  __syncthreads();
-  if (wid == 0) {
-    int s = lane < nw ? warp_acc[lane] : ident;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s = op(s, u);
-    }
-    if (lane < nw) warp_acc[lane] = s;
-  }
-  __syncthreads();
-  int excl = __shfl_up_sync(0xffffffffu, incl, 1);
-  if (lane == 0) excl = ident;
-  if (wid) excl = op(warp_acc[wid - 1], excl);
-  *total = warp_acc[nw - 1];
-  __syncthreads();
-  return excl;
-}
-
 __device__ __forceinline__ uint32_t ue_bits(uint32_t v) { return 2 * (32 - __clz(v + 1)) - 1; }
 
 // mb_skip_run before each coded macroblock (and after the last one when the slice ends in skips), bit offsets, zeroed
@@ -814,34 +768,24 @@ __global__ void __launch_bounds__(kFrameThreads) lspv_offsets_kernel(const Param
   const MbRec* m = mb_recs(p);
   uint32_t* bits = mb_bits(p);
   uint32_t* runs = mb_runs(p);
-  const int per = (p.nmb + kFrameThreads - 1) / kFrameThreads;
-  const int b0 = min(p.nmb, static_cast<int>(threadIdx.x) * per), b1 = min(p.nmb, b0 + per);
+  const bitstream::Chunk c(p.nmb);
   int last = -1;
   if (!p.idr)
-    for (int i = b0; i < b1; ++i)
+    for (int i = c.i0; i < c.i1; ++i)
       if (!m[i].skip) last = i;
   int total;
-  int prev = block_exclusive_scan<true>(last, &total);
-  uint32_t sum = 0;
-  for (int i = b0; i < b1; ++i) {
+  int prev = block_exclusive_scan<Max>(last, &total);
+  const uint32_t end = bitstream::counts_to_offsets(bits, p.nmb, p.sh_bits, [&](int i) -> int {
     uint32_t run = ~0u;
     if (!p.idr) {
       if (!m[i].skip) run = i - prev - 1, prev = i;
       else if (i == p.nmb - 1) run = i - prev;
     }
     runs[i] = run;
-    sum += bits[i] + (run != ~0u ? ue_bits(run) : 0);
-  }
-  int all;
-  uint32_t at = p.sh_bits + block_exclusive_scan<false>(static_cast<int>(sum), &all);
-  for (int i = b0; i < b1; ++i) {
-    const uint32_t b = bits[i] + (runs[i] != ~0u ? ue_bits(runs[i]) : 0);
-    bits[i] = at;
-    at += b;
-  }
-  if (threadIdx.x == 0) bits[p.nmb] = p.sh_bits + static_cast<uint32_t>(all);
+    return run != ~0u ? ue_bits(run) : 0;
+  });
   uint32_t* buf = bit_buf(p);
-  const uint32_t words = (p.sh_bits + static_cast<uint32_t>(all) + 8 + 31) / 32 + 4;
+  const uint32_t words = (end + 8 + 31) / 32 + 4;
   for (uint32_t i = threadIdx.x; i < words; i += kFrameThreads) buf[i] = 0;
 }
 
@@ -851,13 +795,12 @@ __global__ void __launch_bounds__(128) lspv_pack_kernel(const Params p) {
   const MbRec* m = mb_recs(p);
   uint32_t* buf = bit_buf(p);
   if (i == 0) {                                                   // the slice header
-    BitWriter w{buf, 0, 0, 0};
+    BitWriter w(buf, 0);
     for (int k = 0; k < p.sh_bits / 8; ++k) w.put(p.sh[k], 8);
     if (p.sh_bits & 7) w.put(p.sh[p.sh_bits / 8] >> (8 - (p.sh_bits & 7)), p.sh_bits & 7);
     w.flush();
   }
-  const uint32_t off = mb_bits(p)[i];
-  BitWriter w{buf, off >> 5, static_cast<int>(off & 31), 0};
+  BitWriter w(buf, mb_bits(p)[i]);
   const uint32_t run = mb_runs(p)[i];
   if (run != ~0u) put_ue(w, run);
   write_mb(w, p, m, i);
@@ -895,7 +838,7 @@ __global__ void __launch_bounds__(kFrameThreads) lspv_finish_kernel(const Params
       if (at + i < nbytes && bytes[i]) mine = static_cast<int>(at + i);
     }
     int round_last;
-    int prev_nz = max(last_nz, block_exclusive_scan<true>(mine, &round_last));
+    int prev_nz = max(last_nz, block_exclusive_scan<Max>(mine, &round_last));
     uint32_t count = 0;
     int nz = prev_nz;
 #pragma unroll
@@ -906,7 +849,7 @@ __global__ void __launch_bounds__(kFrameThreads) lspv_finish_kernel(const Params
       if (bytes[i]) nz = static_cast<int>(at + i);
     }
     int round_total;
-    int o = base + block_exclusive_scan<false>(static_cast<int>(count), &round_total);
+    int o = base + block_exclusive_scan<Sum>(static_cast<int>(count), &round_total);
     nz = prev_nz;
 #pragma unroll
     for (int i = 0; i < 8; ++i) {
@@ -1024,8 +967,6 @@ int64_t max_bytes_of(int height, int width) {
   const int64_t rbsp = (64 + mbs * mb + 8 + 7) / 8;
   return 2 * 64 + 5 + rbsp + (rbsp + 1) / 2;
 }
-
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 Layout layout_of(int height, int width) {
   const size_t hw = static_cast<size_t>(height) * width, nmb = hw / 256;

@@ -26,9 +26,10 @@ class JpegBatch:
 class JpegEncoder(_lib.Handle):
     """Baseline JPEG encoding of uint8 frames on the device, asynchronous on the current CUDA stream.
 
-    ``encode(images)`` takes ``[n, H, W, 3]`` RGB (tensor2im's layout) or ``[n, H, W]`` grey, H and W multiples of 16;
-    ``encode_into`` writes into caller-owned buffers.  The workspace is kept across calls, so calls of one size allocate
-    nothing that outlives them."""
+    ``encode(images)`` takes ``[n, H, W, 3]`` RGB (tensor2im's layout) or ``[n, H, W]`` grey, H and W multiples of 16,
+    and allocates its outputs and a workspace of its own, so calls on one encoder may run on several CUDA streams at
+    once.  ``encode_into`` writes into caller-owned buffers with a caller-owned workspace, which calls that may overlap
+    must not share."""
     prefix = "lspj"
     what = "the JPEG encoder"
 
@@ -38,7 +39,6 @@ class JpegEncoder(_lib.Handle):
             raise ValueError(f"quality must be in [1, 100] (got {quality})")
         self.quality = int(quality)
         self._create()
-        self._ws = None
 
     def max_bytes(self, height: int, width: int, components: int = 3) -> int:
         """``lspj_max_bytes``: no file of a ``height`` x ``width`` frame is longer."""
@@ -46,25 +46,16 @@ class JpegEncoder(_lib.Handle):
         self.call("max_bytes", int(height), int(width), int(components), C.byref(out))
         return out.value
 
-    @staticmethod
-    def _shape(images: torch.Tensor):
-        if images.dtype != torch.uint8 or not images.is_cuda or images.dim() not in (3, 4) or \
-                (images.dim() == 4 and images.shape[3] != 3):
-            raise ValueError("images must be a uint8 CUDA tensor [n, H, W, 3] (RGB) or [n, H, W] (grey)")
-        n, h, w = images.shape[:3]
-        return int(n), int(h), int(w), 3 if images.dim() == 4 else 1
-
     def encode(self, images: torch.Tensor) -> JpegBatch:
-        n, h, w, c = self._shape(images)
+        n, h, w, c = _lib.frame_shape(images)
         data = torch.empty((n, self.max_bytes(h, w, c)), dtype=torch.uint8, device=self.device)
         sizes = torch.empty(n, dtype=torch.int32, device=self.device)
-        self._ws = _lib.reserve(self._ws, self.workspace_bytes(n, h, w, c), self.device)
-        return self.encode_into(images, data, sizes, self._ws)
+        return self.encode_into(images, data, sizes, self.workspace(n, h, w, c))
 
     def encode_into(self, images: torch.Tensor, out: torch.Tensor, sizes: torch.Tensor, ws: torch.Tensor) -> JpegBatch:
         """Encodes into ``out`` ([>= n, stride] uint8, rows contiguous), ``sizes`` ([>= n] int32) with the workspace ``ws``
         (uint8, at least ``workspace_bytes(n, H, W, components)`` bytes).  Returns the views of the first n rows."""
-        n, h, w, c = self._shape(images)
+        n, h, w, c = _lib.frame_shape(images)
         images = images.contiguous()
         if out.dtype != torch.uint8 or out.dim() != 2 or out.shape[0] < n or out.stride(1) != 1 or \
                 sizes.dtype != torch.int32 or not sizes.is_contiguous() or sizes.shape[0] < n or ws.dtype != torch.uint8:

@@ -108,6 +108,29 @@ def test_pushes_equal_the_whole_clip(push):
     assert whole.is_idr.cpu().tolist() == [1 if i % 60 == 0 else 0 for i in range(70)]
 
 
+def test_two_streams_of_one_encoder_on_two_cuda_streams_equal_their_serial_results():
+    """Each H264Stream owns its workspace, so two streams of one encoder, pushing clips of different sizes on two CUDA
+    streams with nothing ordering one's pushes against the other's, give the bytes and reconstruction of a serial run."""
+    enc = H264Encoder(DEV, qp=26, gop=4, search=8)
+    clips = [torch.from_numpy(clip("noise", 6, 256, 256, seed=1)).to(DEV),
+             torch.from_numpy(clip("translate", 6, 128, 192, seed=2)).to(DEV)]
+    want = []
+    for x in clips:
+        st = enc.stream()
+        want.append((st.push(x).to_bytes(), st.state.cpu()))
+    cuda_streams, streams = [torch.cuda.Stream(DEV) for _ in clips], [enc.stream() for _ in clips]
+    got = [[], []]
+    torch.cuda.synchronize()
+    for at in range(0, 6, 2):
+        for k in (0, 1):
+            with torch.cuda.stream(cuda_streams[k]):
+                got[k].append(streams[k].push(clips[k][at:at + 2]))
+    torch.cuda.synchronize()
+    for k in (0, 1):
+        assert [au for b in got[k] for au in b.to_bytes()] == want[k][0], k
+        assert torch.equal(streams[k].state.cpu(), want[k][1]), k
+
+
 def test_two_runs_give_identical_bytes_under_the_bound():
     frames, _ = _generator_frames(4, 512)
     frames = torch.cat([frames, torch.from_numpy(clip("noise", 2, 512, 512)).to(DEV)])

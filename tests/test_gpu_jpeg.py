@@ -116,18 +116,21 @@ def test_encode_into_makes_no_host_synchronisation():
 
 
 def test_two_streams_equal_their_serial_results():
+    """Two encoders, then one encoder whose two calls differ in batch size: every call has a workspace of its own."""
     a = torch.from_numpy(_images(8, 256, 256, False, 3)).to(DEV)
     b = torch.from_numpy(_images(8, 256, 256, True, 4)).to(DEV)
-    ea, eb = JpegEncoder(DEV, quality=75), JpegEncoder(DEV, quality=95)
-    serial = (ea.encode(a).to_bytes(), eb.encode(b).to_bytes())
-    sa, sb = torch.cuda.Stream(DEV), torch.cuda.Stream(DEV)
-    torch.cuda.synchronize()
-    with torch.cuda.stream(sa):
-        ra = ea.encode(a)
-    with torch.cuda.stream(sb):
-        rb = eb.encode(b)
-    torch.cuda.synchronize()
-    assert (ra.to_bytes(), rb.to_bytes()) == serial
+    shared = JpegEncoder(DEV, quality=75)
+    for (ea, xa), (eb, xb) in (((JpegEncoder(DEV, quality=75), a), (JpegEncoder(DEV, quality=95), b)),
+                               ((shared, a), (shared, b[:3]))):
+        serial = (ea.encode(xa).to_bytes(), eb.encode(xb).to_bytes())
+        sa, sb = torch.cuda.Stream(DEV), torch.cuda.Stream(DEV)
+        torch.cuda.synchronize()
+        with torch.cuda.stream(sa):
+            ra = ea.encode(xa)
+        with torch.cuda.stream(sb):
+            rb = eb.encode(xb)
+        torch.cuda.synchronize()
+        assert (ra.to_bytes(), rb.to_bytes()) == serial
 
 
 def test_encoders_on_two_threads_equal_their_serial_results():
